@@ -2,6 +2,7 @@
 """bench.py -- throughput of the FLAC block encode/decode hot path (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg2|cfg2_l8|cfg3|cfg4|cfg5] [--impl reference]
+                    [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch (BASELINE configs: 10 000 blocks of 4096 samples; cfg4: 125 files
 of 100 blocks per GPU). Prints ONE JSON line (rank 0). See DESIGN.md "Measurement" for the definitions:
@@ -19,7 +20,9 @@ of 100 blocks per GPU). Prints ONE JSON line (rank 0). See DESIGN.md "Measuremen
   frames_compared / frames_equal
              every frame of the GPU stream memcmp'ed against the reference's frame for the same block, in this run.
 Without --workload the default line is cfg2 and the other BASELINE configs ride along under extra.workloads
-(fewer steps), so that one driver invocation measures all of them.
+(same number of steps), so that one driver invocation measures all of them.
+--dump-outputs DIR writes what the device-resident timed path of the headline workload returned in its last timed step
+(see dump_outputs) as DIR/<name>.npy, so that two builds can be compared output for output on identical inputs.
 """
 import argparse
 import json
@@ -128,15 +131,30 @@ def peaks():
     if os.path.exists(p):
         with open(p) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
-def ncu_traffic():
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(p):
-        with open(p) as fh:
-            return json.load(fh)
-    return {}
+DUMP_BYTES = 8 << 20  # bytes of sampled frames / PCM per dump: 32 MB as float32, well under the 64 MB cap
+
+
+def dump_outputs(path, arrays):
+    """Writes each array as path/<name>.npy (float32 / float64)."""
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
+def sample_frames(nframes, frame_cost):
+    """A fixed, seeded choice of frame indices (ascending), as many as fit DUMP_BYTES at frame_cost(i) bytes each."""
+    order = np.random.default_rng(20240607).permutation(nframes)
+    take, total = [], 0
+    for i in order:
+        c = int(frame_cost(int(i)))
+        if total + c > DUMP_BYTES:
+            break
+        take.append(int(i))
+        total += c
+    return np.sort(np.asarray(take, dtype=np.int64))
 
 
 class Ranks:
@@ -192,11 +210,11 @@ def host_threads():
 
 
 # ---------------------------------------------------------------------------------------------- reference (CPU) arm
-def reference_encode_rates(x, bps, rate, level, bs, reps, single_reps=None, one_thread_blocks=400):
-    """The reference libFLAC on this box's host cores over the blocks of x:
-      per_core : one encoder per host thread, contiguous block ranges (ref_encode_parallel), best of `reps`
+def reference_encode_rates(x, bps, rate, level, bs, reps, warmup=1, single_reps=None, one_thread_blocks=400):
+    """The reference libFLAC on this box's host cores over the blocks of x, each figure after `warmup` untimed passes:
+      per_core : one encoder per host thread, contiguous block ranges (ref_encode_parallel), best of `reps` timed passes
       single   : ONE encoder with set_num_threads(min(cores, 64)) -- libFLAC's own multithreading, best of `single_reps`
-      one      : one encoder, one thread, on the first `one_thread_blocks` blocks
+      one      : one encoder, one thread, on the first `one_thread_blocks` blocks, best of `single_reps`
     Msamples/s, samples of all channels."""
     import reflib
     n, ch = x.shape
@@ -204,28 +222,31 @@ def reference_encode_rates(x, bps, rate, level, bs, reps, single_reps=None, one_
     # worker counts tried: every hardware thread, and one per two (physical cores on SMT hosts) -- the better one counts
     best, best_w = None, nt
     for w in sorted({nt, max(1, nt // 2)}, reverse=True):
-        for _ in range(reps + 1):  # first pass is the warm-up
+        for i in range(warmup + reps):
             sec, nfr, _ = reflib.encode_parallel(x, bps, rate, level, bs, w)
             assert nfr == n // bs
-            if best is None or sec < best:
+            if i >= warmup and (best is None or sec < best):
                 best, best_w = sec, w
     out = {"per_core": n * ch / best / 1e6, "cores": nt, "workers": best_w}
     st = min(nt, 64)  # FLAC__STREAM_ENCODER_MAX_THREADS
+    single_reps = single_reps if single_reps is not None else max(1, reps // 2)
     tb = None
-    for _ in range((single_reps if single_reps is not None else max(2, reps // 2)) + 1):
+    for i in range(warmup + single_reps):
         t = time.perf_counter()
         reflib.encode(x, bps, rate=rate, level=level, blocksize=bs, threads=st, md5=False, want_bytes=False)
         dt = time.perf_counter() - t
-        tb = dt if tb is None else min(tb, dt)
+        if i >= warmup:
+            tb = dt if tb is None else min(tb, dt)
     out["single_encoder"] = n * ch / tb / 1e6
     out["single_encoder_threads"] = st
     nb1 = min(one_thread_blocks, n // bs)
     t1 = None
-    for _ in range(2):
+    for i in range(warmup + single_reps):
         t = time.perf_counter()
         reflib.encode(x[: nb1 * bs], bps, rate=rate, level=level, blocksize=bs, threads=1, md5=False, want_bytes=False)
         dt = time.perf_counter() - t
-        t1 = dt if t1 is None else min(t1, dt)
+        if i >= warmup:
+            t1 = dt if t1 is None else min(t1, dt)
     out["one_thread"] = nb1 * bs * ch / t1 / 1e6
     return out
 
@@ -266,7 +287,7 @@ def config_of(name, world):
     cfg = {"workload": f"{name}: {desc}", "channels": ch, "bits_per_sample": bps, "sample_rate": rate,
            "compression_level": level, "blocks_per_gpu_per_step": blocks, "blocksize": bs,
            "sharding": f"{world} rank(s) x independent " + ("files (file index mod world)" if fblocks else "block ranges") + ", no data-path collective",
-           "l2_policy": "inputs (%.0f MB int32/step/GPU) exceed the 126 MB L2" % (blocks * bs * ch * 4 / 1e6)}
+           "l2_policy": "inputs (%.0f MB int32/step/GPU) exceed the 50 MB L2" % (blocks * bs * ch * 4 / 1e6)}
     if fblocks:
         cfg["blocks_per_file"] = fblocks
         cfg["files_per_gpu"] = blocks // fblocks
@@ -280,7 +301,7 @@ def run_reference_arm(args, name):
     config = config_of(name, args.gpus)
     config["blocks_per_gpu_per_step"] = blocks
     nthreads = host_threads()
-    steps = max(args.steps, 5)
+    steps = args.steps
     if name == "cfg5":
         # the reference decoder is single-threaded per stream; every host core decodes its own stream
         # (ctypes releases the GIL), as a many-file batch would
@@ -299,18 +320,18 @@ def run_reference_arm(args, name):
         best = min(times)
         val = nthreads * sample_blocks * bs * ch / best / 1e6
         cpu = {"value": round(val, 3), "unit": "Msamples/s", "cores": nthreads, "kind": "reference",
-               "sample": f"{nthreads} streams x {sample_blocks} frames per step, one reference libFLAC 1.5.0 stream decoder per host thread, MD5 off, in-memory callbacks, best of {steps}"}
+               "sample": f"{nthreads} streams x {sample_blocks} frames per step, one reference libFLAC 1.5.0 stream decoder per host thread, MD5 off, in-memory callbacks, best of {steps} after {args.warmup} untimed"}
         metric, ms = "decode_msamples_per_s", 1e3 * best
     else:
         x = make_pcm(ch, bps, rate, blocks, bs, seed=1)
-        r = reference_encode_rates(x, bps, rate, level, bs, reps=steps)
+        r = reference_encode_rates(x, bps, rate, level, bs, reps=steps, warmup=args.warmup)
         val = r["per_core"]
         ms = blocks * bs * ch / val / 1e3
         cpu = {"value": round(val, 3), "unit": "Msamples/s", "cores": r["cores"], "workers": r["workers"], "kind": "reference",
                "value_single_encoder": round(r["single_encoder"], 3), "single_encoder_threads": r["single_encoder_threads"],
                "value_1_thread": round(r["one_thread"], 3),
                "sample": f"all {blocks} blocks of the workload per step, reference libFLAC 1.5.0 (oracle/_ref, shipped flags), one encoder per host thread "
-                         f"over contiguous block ranges, MD5 off, in-memory callbacks, best of {steps}; value_single_encoder = one encoder with set_num_threads"}
+                         f"over contiguous block ranges, MD5 off, in-memory callbacks, best of {steps} after {args.warmup} untimed; value_single_encoder = one encoder with set_num_threads"}
         metric = "encode_msamples_per_s"
     return {"impl": "reference", "metric": metric, "value": round(val, 3), "unit": "Msamples/s", "n_gpus": args.gpus,
             "steps": steps, "warmup": args.warmup, "ms_per_step": round(ms, 3), "higher_is_better": True, "scaling": "weak",
@@ -319,7 +340,7 @@ def run_reference_arm(args, name):
             "gpu_launches": 0}
 
 
-# ---------------------------------------------------------------------------------------------- B200 arm: decode
+# ---------------------------------------------------------------------------------------------- GPU arm: decode
 def bench_decode(args, ranks, name, steps, warmup, with_cpu):
     import ctypes as C
     import torch
@@ -388,6 +409,12 @@ def bench_decode(args, ranks, name, steps, warmup, with_cpu):
     ranks.barrier()
     dev_ms = ranks.max(ev0.elapsed_time(ev1))
     launches = dec.launches - launches0
+    if args.dump_outputs and rank == 0:
+        # decoded PCM of a seeded sample of frames (int32 samples of <= 24 bits are exact in float32) and every frame's status
+        idx = sample_frames(blocks, lambda i: 4 * bs * ch)
+        pcm = d_pcm.view(blocks, bs, ch)[torch.from_numpy(idx).to(d_pcm.device)]
+        dump_outputs(args.dump_outputs, {"pcm_sample": pcm.cpu().numpy().astype(np.float32), "pcm_sample_frames": idx.astype(np.float64),
+                                         "frame_status": d_status.cpu().numpy().astype(np.float64)})
     prof = dec.profile(reset=True)
     dec.set_profiling(False)
 
@@ -402,9 +429,9 @@ def bench_decode(args, ranks, name, steps, warmup, with_cpu):
     step_host_int32()
     ranks.barrier()
     t0 = time.perf_counter()
-    for _ in range(max(2, steps // 2)):
+    for _ in range(steps):
         step_host_int32()
-    e2e32_s = ranks.max(time.perf_counter() - t0) / max(2, steps // 2)
+    e2e32_s = ranks.max(time.perf_counter() - t0) / steps
     ranks.barrier()
     clocks = sampler.stop() if rank == 0 else None
     assert np.array_equal(h_pcm.numpy(), x), "e2e decoded PCM (int32) differs from the input"
@@ -433,9 +460,8 @@ def bench_decode(args, ranks, name, steps, warmup, with_cpu):
                           "frac": round(alg / (avg_ms * 1e-3) / 1e9 / peak, 4)}
     dominant = max(kernels, key=lambda k: kernels[k]["share"])
     dk = kernels[dominant]
-    traffic = ncu_traffic().get(name, {})
     roofline = {"kernel": dominant, "bound": "hbm", "achieved": dk["achieved_gbs"], "peak": peak, "unit": "GB/s", "frac": dk["frac"],
-                "traffic": traffic.get(dominant), "peak_source": peak_src, "share_of_step": dk["share"],
+                "peak_source": peak_src, "share_of_step": dk["share"],
                 "pipeline": {"alg_bytes_per_step": int((frame_bytes + 4 * bs * ch) * blocks),
                              "achieved_gbs": round((frame_bytes + 4 * bs * ch) * blocks * steps / (dev_ms * 1e-3) / 1e9, 2)},
                 "kernels": kernels}
@@ -471,7 +497,7 @@ def bench_decode(args, ranks, name, steps, warmup, with_cpu):
     }
 
 
-# ---------------------------------------------------------------------------------------------- B200 arm: encode
+# ---------------------------------------------------------------------------------------------- GPU arm: encode
 def bench_encode(args, ranks, name, steps, warmup, with_cpu):
     import torch
     import flac_b200
@@ -537,6 +563,13 @@ def bench_encode(args, ranks, name, steps, warmup, with_cpu):
     ranks.barrier()
     dev_ms = ranks.max(ev0.elapsed_time(ev1))
     launches = enc.launches - launches0
+    if args.dump_outputs and rank == 0:
+        # every frame offset (exact in float64) and the bytes of a seeded sample of whole frames, concatenated in frame order
+        offs = d_offs.cpu().numpy()
+        idx = sample_frames(blocks, lambda i: offs[i + 1] - offs[i])
+        sel = torch.cat([d_out[int(offs[i]):int(offs[i + 1])] for i in idx]).cpu().numpy()
+        dump_outputs(args.dump_outputs, {"frame_offsets": offs.astype(np.float64), "frame_bytes_sample": sel.astype(np.float32),
+                                         "frame_bytes_sample_frames": idx.astype(np.float64)})
     # ---- the same K steps again with CUDA events recorded BETWEEN the kernels (per-kernel durations for the roofline; the
     # events serialise the two kernels the engine otherwise overlaps, so this pass is a little slower than the timed one)
     enc.set_profiling(True)
@@ -636,16 +669,12 @@ def bench_encode(args, ranks, name, steps, warmup, with_cpu):
                      "k_emit": "k_emit3"} if emit_direct else
                     {"k_prep": "k_prep", "k_autoc": "k_autoc3 / k_autoc", "k_lpc": "k_lpc", "k_search": "k_search5 / k_search", "k_emit": "k_emit", "k_scan": "k_scan",
                      "k_gather": "k_gather"})
-    traffic_per_block = ncu_traffic().get(name, {})
-    traffic = {}
     total_kernel_ms = sum(v[0] for v in prof.values()) or 1.0
     kernels = {}
     for kname, (ms, n) in prof.items():
         if n == 0 or ms / n < 0.004:  # an empty profiling slot (no kernel between its two events)
             continue
         blocks_per_launch = blocks * steps / n
-        if isinstance(traffic_per_block.get(kname), (int, float)):
-            traffic[kname] = int(traffic_per_block[kname] * blocks_per_launch)
         alg = per_block_bytes[kname] * blocks_per_launch
         avg_ms = ms / n
         kernels[kname] = {"ms_per_launch": round(avg_ms, 4), "launches": n, "share": round(ms / total_kernel_ms, 4),
@@ -654,7 +683,7 @@ def bench_encode(args, ranks, name, steps, warmup, with_cpu):
     dominant = max(kernels, key=lambda k: kernels[k]["share"])
     dk = kernels[dominant]
     roofline = {"kernel": dominant, "bound": "hbm", "achieved": dk["achieved_gbs"], "peak": peak, "unit": "GB/s", "frac": dk["frac"],
-                "traffic": traffic.get(dominant), "peak_source": peak_src, "share_of_step": dk["share"],
+                "peak_source": peak_src, "share_of_step": dk["share"],
                 "residual_rice_kernel": {"kernel": "k_emit3" if emit_direct else "k_emit", **kernels.get("k_emit", {})},
                 "pipeline": {"alg_bytes_per_step": int((4 * bs * ch + frame_bytes) * blocks),
                              "achieved_gbs": round((4 * bs * ch + frame_bytes) * blocks * steps / (dev_ms * 1e-3) / 1e9, 2)},
@@ -671,8 +700,8 @@ def bench_encode(args, ranks, name, steps, warmup, with_cpu):
                 cpu = {"value": round(r["per_core"], 3), "unit": "Msamples/s", "cores": r["cores"], "workers": r["workers"], "kind": "reference",
                        "value_single_encoder": round(r["single_encoder"], 3), "single_encoder_threads": r["single_encoder_threads"],
                        "value_1_thread": round(r["one_thread"], 3),
-                       "sample": f"all {blocks} blocks of this workload, reference libFLAC 1.5.0 built from /root/reference (oracle/_ref, shipped flags), one encoder per "
-                                 f"host thread over contiguous block ranges, MD5 off, in-memory callbacks, best of 3-5 (the --impl reference procedure)"}
+                       "sample": f"all {blocks} blocks of this workload, reference libFLAC 1.5.0 (oracle/_ref, shipped flags), one encoder per "
+                                 f"host thread over contiguous block ranges, MD5 off, in-memory callbacks, best of 3-5 after one untimed pass (the --impl reference procedure)"}
         except Exception as ex:  # the baseline is reported, never required for the GPU number
             cpu = {"value": None, "unit": "Msamples/s", "cores": 0, "kind": "reference", "sample": f"unavailable: {ex}"}
 
@@ -722,6 +751,8 @@ def main():
     ap.add_argument("--kernels-only", action="store_true", help="profiling aid: device-resident steps only (no e2e, no CPU baseline)")
     ap.add_argument("--no-extras", action="store_true", help="default invocation: only the cfg2 line, no extra.workloads")
     ap.add_argument("--full-cpu", action="store_true", help="cpu_baseline with best of 5 instead of 3")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline workload's outputs of its last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else max(args.warmup, 1)
     primary = args.workload or "cfg2"
@@ -734,7 +765,7 @@ def main():
         print(json.dumps(run_reference_arm(args, primary)))
         return 0
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     import torch
     if not torch.cuda.is_available():
         print(json.dumps({"error": "no CUDA device: flac_b200 has no CPU fallback"}))
@@ -747,19 +778,19 @@ def main():
         return fn(args, ranks, name, steps, warmup, with_cpu)
 
     line = run(primary, args.steps, args.warmup, True)
+    args.dump_outputs = None  # the dump is the headline workload's
     if args.workload is None and not args.no_extras and not args.kernels_only:
         extras = {}
-        xsteps = max(3, args.steps // 4)
         for name in ("cfg2_l8", "cfg3", "cfg4", "cfg5"):
             try:
-                extras[name] = summarize(run(name, xsteps, 3, True))
+                extras[name] = summarize(run(name, args.steps, args.warmup, True))
             except AssertionError:
                 raise
             except Exception as ex:  # an extra must never take the headline line down
                 extras[name] = {"error": f"{type(ex).__name__}: {ex}"}
         if ranks.rank == 0:
             line["extra"] = {"workloads": extras,
-                             "note": "the other BASELINE configs, same procedure, fewer timed steps; parity counted per workload"}
+                             "note": "the other BASELINE configs, same procedure and steps; parity counted per workload"}
     if ranks.rank == 0:
         print(json.dumps(line))
     ranks.close()

@@ -1,7 +1,7 @@
-"""flac_b200 -- B200-native FLAC block encode/decode engine.
+"""flac_b200 -- H100-native FLAC block encode/decode engine.
 
 This package is only the host-side Python mirror of the C ABI in include/flac_b200.h
-(libflac_b200.so: hand-written sm_100a CUDA kernels + host C++). There is no CPU fallback:
+(libflac_b200.so: hand-written sm_90a CUDA kernels + host C++). There is no CPU fallback:
 if the shared library is missing or no CUDA device is present every compute call raises.
 
 Names mirror the reference's encoder/decoder interface (FLAC__stream_encoder_set_* knobs

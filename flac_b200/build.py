@@ -1,4 +1,4 @@
-"""Builds flac_b200/libflac_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds flac_b200/libflac_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m flac_b200.build [--force]
 
@@ -19,7 +19,7 @@ HDR = sorted(glob.glob(os.path.join(HERE, "csrc", "*.h")) + glob.glob(os.path.jo
 OUT = os.path.join(HERE, "libflac_b200.so")
 
 NVCC_FLAGS = [
-    "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-fmad=false",
+    "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-fmad=false",
     "-Xcompiler", "-fPIC,-ffp-contract=off,-fvisibility=default",
 ]
 

@@ -1,17 +1,16 @@
 // autoc_kernel.cuh -- k_autoc3: windowed FP64 autocorrelation, one warp per 32 chains,
 // samples staged through shared memory with an asynchronous multi-stage copy pipeline.
 //
-// What bounds this kernel (tools/ubench/fp64_rates.cu, measured on B200): DFMA issues at
-// 64 lanes/clk/SM (2 cycles per warp instruction per SM sub-partition), a dependent DFMA takes
-// ~10.7 cycles, F2F.F64.F32 runs at 16 lanes/clk/SM on its own pipe.  A chain (one section of
+// What bounds this kernel (tools/ubench/fp64_rates.cu measures these rates): the DFMA issue rate,
+// the latency of a dependent DFMA, and F2F.F64.F32 on its own, slower pipe.  A chain (one section of
 // one signal) must add its lag products in ascending sample order (lpc.c:121-140 sums that way
 // and every partial sum is rounded), so the only parallelism is ACROSS chains and across the
 // LAGS accumulators of one chain.  One thread therefore owns one chain with all its lags in
 // registers (LAGS independent DFMA chains >= the 6 needed to cover the DFMA latency), and the
 // job of the rest of the kernel is to keep that thread from ever waiting on memory: k_autoc2
-// (thread-private 128-bit global loads, one predicated window load per sample) spent ~230
-// cycles per sample against ~2*LAGS for the arithmetic, because with at most a few warps per
-// sub-partition nothing hides a load.
+// (thread-private 128-bit global loads, one predicated window load per sample) spent most of
+// its cycles waiting on loads, because with at most a few warps per sub-partition nothing
+// hides a load.
 //
 // Layout: CTA = one warp = 32 consecutive items of ONE section (so window indices, tile
 // counts and all control flow are warp-uniform).  Per tile of T samples the warp issues
@@ -63,8 +62,8 @@ __global__ void __launch_bounds__(32) k_autoc3(EncK P, const int32_t *__restrict
 
 	const int lane = threadIdx.x;
 	// section slowest: the longest chains (full-length sections) start first. (Section-fastest ordering would let L2
-	// serve the partial-window re-reads -- DRAM traffic is 2.7x the unique bytes at -8 -- but measured 24 % slower:
-	// the kernel is FP64-bound and the long chains then finish last.)
+	// serve the partial-window re-reads, which multiply DRAM traffic at -8, but it was measured slower on the GPU this
+	// kernel was first tuned on, not on H100: the kernel is FP64-bound and the long chains then finish last.)
 	const int groups = (nitems + 31) >> 5;
 	const int sec = blockIdx.x / groups;
 	const int item0 = (blockIdx.x - sec * groups) << 5;

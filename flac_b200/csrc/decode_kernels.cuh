@@ -1,10 +1,10 @@
-// decode_kernels.cuh -- sm_100a kernels of the FLAC batch frame decoder.
+// decode_kernels.cuh -- sm_90a kernels of the FLAC batch frame decoder.
 //
 // Frames carry no length field and Rice codes have data-dependent lengths: where subframe c+1 starts is only known
 // once subframe c has been walked, and the LPC restore is a serial recurrence (SURVEY.md 7.3-6). Round 1 ran the whole
 // frame in one thread (header, every subframe, Rice decode fused with the restore, planar scratch, then a merge pass):
-// 89 % of the decode step at 2.6 % of HBM, divergent (32 different frames per warp, each in a different loop nest) and
-// with 4-byte stores 16 KB apart. This generation splits the frame along its only parallel axis, the channels:
+// most of the decode step at a small fraction of HBM bandwidth, divergent (32 different frames per warp, each in a
+// different loop nest) and with 4-byte stores 16 KB apart. This generation splits the frame along its only parallel axis, the channels:
 //   k_dec_walk   : one thread per frame -- header (stream_decoder.c:2624-2947) + CRC-8, then a WALK over subframes
 //                  0..channels-2 that only measures them (unary length + k per code, no sample is formed): the bit
 //                  offset of every subframe. ~10 instructions per code.
@@ -71,8 +71,9 @@ struct DecSubframeInfo {
 // (~5 Rice codes of the whole warp) cover an L2 hit, and whenever the reader enters a new 128-byte line it prefetches the line
 // after the next into L2. Consuming bits is an add and a test; only a word crossing (every ~2.5 codes) moves registers and
 // loads. Words past `nwords` read as zeros: no read leaves the frame's last 16-byte granule. (Earlier versions, for the
-// record: one dependent 32-bit load per refill = ~250 cycles per Rice code; a three-deep queue of 128-bit loads whose
-// rotation cost 5 moves per word; a 64-bit left-aligned accumulator whose branch-free refill cost ~14 instructions per code.)
+// record: one dependent 32-bit load per refill, i.e. a full load latency per Rice code; a three-deep queue of 128-bit loads
+// whose rotation cost 5 moves per word; a 64-bit left-aligned accumulator whose branch-free refill cost many instructions per
+// code.)
 struct BitRd {
 	const uint32_t *words;         // 128-byte aligned address at or below the frame's first byte
 	uint32_t nwords;               // words (from `words`) that may be read
@@ -387,7 +388,7 @@ __global__ void __launch_bounds__(128) k_dec_walk(DecK P, const uint8_t *__restr
 // is unrolled MAXORD times so that every history access has a compile-time register index.
 // The rare events of the sample loop live out of line (by value in, by value out: the reader stays in registers on the hot path):
 // the loop body is unrolled MAXORD times, and with every slow path inlined at every site it outgrew the instruction cache
-// (18 % of the stall samples were instruction fetches).
+// (instruction fetches showed up among the stall reasons).
 struct DecPart {
 	uint32_t k, raw, next_part, part_end, esc;
 };

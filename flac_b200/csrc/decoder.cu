@@ -1,4 +1,4 @@
-// decoder.cu -- host side of the B200 FLAC batch frame decoder + its C ABI (include/flac_b200.h).
+// decoder.cu -- host side of the FLAC batch frame decoder + its C ABI (include/flac_b200.h).
 #include <string.h>
 
 #include <algorithm>
@@ -261,7 +261,7 @@ static int decode_host_impl(fb200_decoder *d, const uint8_t *frames, const uint6
 	}
 	if(!d->s_h2d) FB_CUDA(cudaStreamCreateWithFlags(&d->s_h2d, cudaStreamNonBlocking));
 	if(!d->s_d2h) FB_CUDA(cudaStreamCreateWithFlags(&d->s_d2h, cudaStreamNonBlocking));
-	// chunks: 16 per call, at least 1024 frames, at most the launch capacity
+	// chunks: 16 per call, at least 1024 frames, at most the launch capacity (chosen on a previous GPU, not re-measured on H100)
 	uint32_t chunk = (nframes + 15) / 16;
 	if(chunk < 1024) chunk = 1024;
 	if(chunk > d->max_frames) chunk = d->max_frames;
@@ -384,7 +384,9 @@ int fb200_decoder_index_host(fb200_decoder *d, const uint8_t *stream, uint64_t n
 	FB_CUDA(cudaMemcpyAsync(d->d_stream, stream, nbytes, cudaMemcpyHostToDevice, d->stream));
 	FB_CUDA(cudaMemsetAsync(d->d_stream + nbytes, 0, 64, d->stream));
 	FB_CUDA(cudaMemsetAsync(d->d_count, 0, sizeof(unsigned), d->stream));
-	k_dec_scan<<<148 * 8, 256, 0, d->stream>>>(d->d_stream, nbytes, d->d_cand, capacity, d->d_count);
+	int nsm = 0;
+	FB_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, d->device));
+	k_dec_scan<<<nsm * 8, 256, 0, d->stream>>>(d->d_stream, nbytes, d->d_cand, capacity, d->d_count);
 	d->launches++;
 	unsigned n = 0;
 	FB_CUDA(cudaMemcpyAsync(&n, d->d_count, sizeof n, cudaMemcpyDeviceToHost, d->stream));

@@ -196,8 +196,8 @@ __device__ __forceinline__ int fixed_tap(int order, int j)
 // MASKED: leave out the first ord0 outputs (the warm-up samples of the block's very first group;
 // order <= MAXORD <= ... so only outputs m < MAXORD can be masked).
 // The body is deliberately small (G x NTAPS MACs): the callers loop over groups with a ROLLED loop so
-// the hot code stays inside the instruction cache (a fully unrolled 32 x 12 run per variant did not:
-// ncu showed 30 % "no_instructions" stalls).
+// the hot code stays inside the instruction cache (a fully unrolled 32 x 12 run per variant did not: the
+// profiler showed warps stalled on instruction fetch).
 template <int G, int MAXORD, int NTAPS, bool WIDE, bool MASKED, bool NARROW>
 __device__ __forceinline__ void group_abs_sum(const int (&xg)[MAXORD + G], const int (&q)[MAXORD], int shift, int ord0, int limit,
                                               uint32_t &s32, unsigned long long &s64, bool &bad)

@@ -7,10 +7,9 @@
 // FLAC__bitwriter_write_rice_signed_block (bitwriter.c:575-706), zero pad + CRC-16 (stream_encoder.c:3465-3480,
 // crc.c:376-396), channel assignment argmin (stream_encoder.c:3937-3972).
 //
-// What round 1's k_emit2 spent its time on (ncu, profiles/r1g_full_cfg2.csv): ~158 thread-instructions per
-// sample, 31 % of the stall samples at block barriers (14+ barriers per frame: one exclusive scan and one
-// re-staging per channel), 11.6 M shared-memory bank conflicts, a byte-at-a-time CRC, a worst-case zero fill and
-// a slot -> gather double copy.  This kernel:
+// What round 1's k_emit2 spent its time on (profiled): many thread-instructions per sample, stalls at block
+// barriers (14+ barriers per frame: one exclusive scan and one re-staging per channel), shared-memory bank
+// conflicts, a byte-at-a-time CRC, a worst-case zero fill and a slot -> gather double copy.  This kernel:
 //   * stages the caller's interleaved int32 block ONCE with a 1-D TMA bulk copy (cp.async.bulk + mbarrier), forms
 //     the two signals the channel assignment picked (L/R/M/S, wasted bits shifted out) in place;
 //   * a thread owns one run of R_T consecutive samples of one channel (row layout of k_search4: 36-word rows ->

@@ -1,4 +1,4 @@
-// encode_kernels.cuh -- sm_100a kernels of the FLAC block encoder.
+// encode_kernels.cuh -- sm_90a kernels of the FLAC block encoder.
 //
 // Pipeline for a launch of N equal-sized blocks (frames are independent: SURVEY.md §0.1):
 //   k_prep    : de-interleave, mid/side, wasted bits            (stream_encoder.c:3777-3867)
@@ -250,8 +250,8 @@ __device__ __forceinline__ double expected_bits_scale(double lpc_error, double e
 // lpc.c:176-218 FLAC__lpc_compute_lp_coefficients. Runs the recursion up to max_order (or until the error hits 0.0),
 // records the error per order and, when want_order > 0, the float predictor coefficients of that order. Returns the
 // effective max order. Every loop is unrolled to the template bound MO with the live range as a predicate, so the
-// working arrays stay in registers (round 1's run-time indexed version kept 1 KB of them in local memory per thread:
-// 52 % long-scoreboard stalls). The arithmetic -- operations and their order -- is the reference's, statement by statement.
+// working arrays stay in registers (round 1's run-time indexed version kept 1 KB of them in local memory per thread
+// and stalled on those loads). The arithmetic -- operations and their order -- is the reference's, statement by statement.
 template <int MO>
 __device__ __forceinline__ int levinson(const double (&ac)[MO + 1], int max_order, int want_order, double (&err_out)[MO], float (&coef_out)[MO])
 {

@@ -1,4 +1,4 @@
-// encoder.cu -- host side of the B200 FLAC block encoder + its C ABI (include/flac_b200.h).
+// encoder.cu -- host side of the FLAC block encoder + its C ABI (include/flac_b200.h).
 //
 // The host does what the reference does once per (encoder, blocksize): validate settings
 // (init_stream_internal_, src/libFLAC/stream_encoder.c:725-830), generate the apodization
@@ -113,9 +113,10 @@ struct fb200_encoder {
 	unsigned long long *h_totals = nullptr;  // pinned
 	size_t h_totals_cap = 0;
 	uint64_t launches = 0;
-	int host_chunks = 12;   // chunks per fb200_encode_host call (FB200_HOST_CHUNKS): copy/compute overlap granularity; measured best 8-12 (tools/sweep_host_chunks.py)
+	int host_chunks = 12;   // chunks per fb200_encode_host call (FB200_HOST_CHUNKS): copy/compute overlap granularity; on an H100 SXM at 400 W
+	                        // (tools/sweep_host_chunks.py, packed 16-bit, 10 000 blocks) 8-16 are equal within noise and 4 / 24 are ~7 % slower at -8
 	int pipe_chunks = 1;    // sub-batches per fb200_encode_device call (FB200_PIPE_CHUNKS); see fb200_encode_device
-	int f64b = 0;         // FB200_SEARCH_F64B=1: the second warp of a signal runs on the FP64 pipe (measured SLOWER: -8 2.59 vs 2.02 ms; kept for A/B)
+	int f64b = 0;         // FB200_SEARCH_F64B=1: the second warp of a signal runs on the FP64 pipe (slower: H100 SXM at 400 W, -8, 10 000 blocks: 4.48 vs 3.89 ms per step; kept for A/B)
 	int debug_path = 0;   // FB200_DEBUG_PATH bit mask (bisecting aid): 1 = k_prep + k_autoc3 instead of k_autoc4, 2 = general search, 4 = general emit, 8 = k_meta instead of the OR fused into k_autoc4
 	bool use_v1 = false;  // FB200_FORCE_GENERAL_KERNELS=1: run the general kernels for every blocksize (tests)
 	// optional per-kernel CUDA-event timing (bench.py's roofline numbers)
@@ -477,7 +478,7 @@ static int fork_stage_a(fb200_encoder *e, cudaStream_t st)
 
 extern "C" {
 
-const char *fb200_version(void) { return "flac_b200 0.1 (sm_100a)"; }
+const char *fb200_version(void) { return "flac_b200 0.1 (sm_90a)"; }
 const char *fb200_last_error(void) { return fb200::get_error(); }
 
 int fb200_device_count(void)
@@ -732,7 +733,9 @@ int fb200_encoder_create(const fb200_encoder_config *cfg_in, int device, uint32_
 	}
 	{
 		// dynamic shared-memory opt-ins are per function and per device: raised once to fixed maxima, never per encoder
-		// (two encoders with different blocksizes in one process must not lower each other's limit)
+		// (two encoders with different blocksizes in one process must not lower each other's limit). The maxima (160 KB for
+		// k_autoc4, 200 KB for k_search5 / k_emit3 / k_join) and the kernels' launch shapes were chosen on a previous GPU
+		// and carried over unmeasured: they fit H100's 227 KB per block, and its per-SM registers and shared memory are the same.
 		static bool inited[64] = {false};
 		if(device < 64 && !inited[device]) {
 			general_kernels_init(device);
@@ -817,9 +820,10 @@ int fb200_encode_device(fb200_encoder *e, const int32_t *d_pcm, uint64_t samples
 	unsigned long long *offs = reinterpret_cast<unsigned long long *>(d_frame_offsets);
 	if(samples == 0) FB_CUDA(cudaMemsetAsync(offs, 0, sizeof(unsigned long long), st));
 	// Sub-batches of at most max_blocks blocks; stage A (prep/autoc/lpc) of one overlaps stage B (search/emit) of the
-	// previous on a second stream. Measured (tools/sweep_chunks.sh, 10 000 blocks): one launch set per call is fastest
-	// (-5: 1.85 ms vs 2.02 ms with 4 sub-batches; -8: 4.62 vs 4.87) -- every kernel is more efficient at full batch
-	// size than the overlap wins back, so the default is as few sub-batches as the workspace allows.
+	// previous on a second stream. Measured on an H100 SXM at 400 W (tools/sweep_chunks.sh, 10 000 blocks): one launch set
+	// per call is fastest at -5 (1.24 ms per step vs 1.34 with 4 sub-batches) and no sub-batch count wins at -8 (3.83-3.89 ms for
+	// 1-4) -- every kernel is more efficient at full batch size than the overlap wins back, so the default is as few
+	// sub-batches as the workspace allows.
 	uint64_t chunk = (nfull + e->pipe_chunks - 1) / e->pipe_chunks;
 	if(chunk < 512) chunk = 512;
 	if(chunk > e->max_blocks) chunk = e->max_blocks;

@@ -1,10 +1,9 @@
 // search_kernel.cuh -- k_search5: one CTA per block, two warps per signal, register-resident partition tree.
 //
-// ncu on k_search3 at -8 (profiles/r1c_*): the FIR taps were 37 % of the instructions but only
-// 28 % of the time; 40 % went into the per-candidate tail (zeroing / read-modify-write of a
-// shared-memory heap, six barrier-separated merge levels, four chunked parameter sweeps with
-// 64-bit shared traffic) and 19 % into group-loop control (a jump-table switch and ~50
-// address instructions per 16-output group).  This generation keeps the arithmetic and the
+// Profiling k_search3 at -8 showed the FIR taps taking the smaller part of the time; most went into
+// the per-candidate tail (zeroing / read-modify-write of a shared-memory heap, six barrier-separated
+// merge levels, four chunked parameter sweeps with 64-bit shared traffic) and into group-loop control
+// (a jump-table switch and dozens of address instructions per 16-output group).  This generation keeps the arithmetic and the
 // decision order (stream_encoder.c:4191-4269, 4701-5075) and changes the mechanics:
 //   * the predictor class (taps x width) is chosen ONCE per candidate; the tile/group loops are
 //     straight pointer walks (a zeroed row in front of the signal removes the row-0 branch);
@@ -19,8 +18,8 @@
 
 namespace fb200 {
 
-// The 64-bit-accumulator predictor (lpc.c:786-884, subframes deeper than 16 bits) on the FP64 pipe. Measured on
-// B200 (tools/ubench): IMAD.WIDE chains run at ~13 lanes/clk/SM, DFMA at ~57. Everything here is an integer
+// The 64-bit-accumulator predictor (lpc.c:786-884, subframes deeper than 16 bits) on the FP64 pipe: IMAD.WIDE
+// chains issue several times slower than DFMA (tools/ubench measures both). Everything here is an integer
 // below 2^51 held in a double, so every operation is exact: qd[j] = q[j] * 2^-shift (a power-of-two scaling keeps
 // the significand), sum = sum_j qd[j] x[i-1-j] = (integer sum) / 2^shift, floor(sum) by adding 1.5 * 2^52 rounding
 // down (== the reference's arithmetic right shift), |residual| added into a double (< 2^45 per run).

@@ -210,7 +210,7 @@ uint32_t batch_blocks()
 extern "C" {
 
 const char *FLAC__VERSION_STRING = "1.5.0-b200";
-const char *FLAC__VENDOR_STRING = "flac_b200 0.1 (libFLAC 1.5.0 bitstream, sm_100a)";
+const char *FLAC__VENDOR_STRING = "flac_b200 0.1 (libFLAC 1.5.0 bitstream, sm_90a)";
 
 const char *const FLAC__StreamEncoderStateString[] = {
 	"FLAC__STREAM_ENCODER_OK", "FLAC__STREAM_ENCODER_UNINITIALIZED", "FLAC__STREAM_ENCODER_OGG_ERROR",

@@ -1,5 +1,5 @@
 /*
- * flac_b200.h -- C ABI of the B200-native FLAC block engine (libflac_b200.so).
+ * flac_b200.h -- C ABI of the H100-native FLAC block engine (libflac_b200.so).
  *
  * Plain pointers and sizes only. This is the boundary the reference's per-frame hot path
  * is replaced at: everything libFLAC does between "a blocksize worth of samples is

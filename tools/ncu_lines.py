@@ -1,7 +1,7 @@
 """Attribute an ncu source-page (SASS) export to CUDA source lines using nvdisasm line info.
 
     ncu -i rep.ncu-rep --page source --csv --kernel-name regex:k_search3 > sass.csv
-    cuobjdump -xelf all libflac_b200.so ; nvdisasm -g -c encoder.sm_100a.cubin > dis.txt
+    cuobjdump -xelf all libflac_b200.so ; nvdisasm -g -c encoder.sm_90a.cubin > dis.txt
     python tools/ncu_lines.py sass.csv[.gz] dis.txt <mangled-function-name> [top] [kernel-name-substring]
 
 With several kernels in one export, the last argument picks the launch whose demangled name contains it (default: first).

@@ -1,5 +1,5 @@
 // Micro-benchmark: FP64 / conversion pipe rates and latencies on this GPU (inputs to k_autoc's roofline).
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o fp64_rates fp64_rates.cu && ./fp64_rates
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o fp64_rates fp64_rates.cu && ./fp64_rates
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -58,7 +58,7 @@ int main()
 	const double mhz = khz / 1000.0;
 	printf("%s  SMs=%d  clock=%.0f MHz\n", p.name, p.multiProcessorCount, mhz);
 	double *d_out; float *d_in;
-	cudaMalloc(&d_out, sizeof(double) * 148 * 8 * 1024 * 2);
+	cudaMalloc(&d_out, sizeof(double) * p.multiProcessorCount * 8 * 1024 * 2);
 	float h[16]; for(int i = 0; i < 16; i++) h[i] = 1.0f + i * 1e-3f;
 	cudaMalloc(&d_in, sizeof h); cudaMemcpy(d_in, h, sizeof h, cudaMemcpyHostToDevice);
 	const int sms = p.multiProcessorCount;
