@@ -60,6 +60,15 @@ class SubframePlan(C.Structure):
     ]
 
 
+class CandDesc(C.Structure):
+    """Mirror of fb200::CandDesc: one LPC candidate slot of k_lpc (debug_lpc)."""
+    _fields_ = [
+        ("valid", C.c_int32), ("order", C.c_int32), ("precision", C.c_int32), ("shift", C.c_int32),
+        ("wide", C.c_int32), ("limit", C.c_int32), ("pad0", C.c_int32), ("pad1", C.c_int32),
+        ("qlp", C.c_int32 * MAX_LPC_ORDER),
+    ]
+
+
 class SubframeInfo(C.Structure):
     """Mirror of fb200_subframe_info (what FLAC__Frame.subframes[] carries)."""
     _fields_ = [("type", C.c_uint8), ("order", C.c_uint8), ("wasted_bits", C.c_uint8), ("qlp_coeff_precision", C.c_uint8),
@@ -292,6 +301,12 @@ def lib():
     L.fb200_encoder_get_profile.restype = C.c_int
     L.fb200_encoder_get_profile.argtypes = [C.c_void_p, C.POINTER(C.c_double * 7), C.POINTER(C.c_uint64 * 7), C.c_int]
     L.fb200_debug_copy_plans.restype = C.c_int
+    L.fb200_debug_evaluate_lpc.restype = C.c_int
+    L.fb200_debug_evaluate_lpc.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32, C.c_uint32,
+                                           C.c_uint32, C.c_uint32, C.c_void_p]
+    L.fb200_debug_lpc.restype = C.c_int
+    L.fb200_debug_lpc.argtypes = [C.c_int, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32,
+                                  C.c_uint32, C.c_int, C.c_int, C.c_uint32, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_uint32)]
     L.fb200_debug_copy_plans.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p]
     if hasattr(L, "fb200_decoder_create"):
         L.fb200_decoder_create.restype = C.c_int
@@ -521,6 +536,41 @@ def replaygain_device(d_pcm_ptr, pcm_values, files, device=0, stream=0):
     info = (ReplayGainInfo * max(len(files), 1))()
     _check(lib().fb200_replaygain_device(device, d_pcm_ptr, pcm_values, arr, len(files), info, C.c_void_p(stream)))
     return list(info[:len(files)])
+
+
+def debug_evaluate_lpc(signals, meta, cands, min_po, max_po, rice_limit, device=0):
+    """Test hook fb200_debug_evaluate_lpc: the general search kernel's estimate of cands[i] (int32 [n, 40] CandDesc words, as
+    debug_lpc returns them) on signals[i] (int32 [n, blocksize]) with meta[i] = (wasted bits, subframe bps); 0xffffffff when
+    the candidate is rejected."""
+    s = np.ascontiguousarray(signals, dtype=np.int32)
+    m = np.ascontiguousarray(meta, dtype=np.int32).reshape(-1, 2)
+    c = np.ascontiguousarray(cands, dtype=np.int32).reshape(-1, C.sizeof(CandDesc) // 4)
+    n, bs = s.shape
+    assert m.shape[0] == n and c.shape[0] == n
+    est = np.zeros(n, dtype=np.uint32)
+    _check(lib().fb200_debug_evaluate_lpc(device, s.ctypes.data, m.ctypes.data, c.ctypes.data, C.sizeof(CandDesc), n, bs, min_po, max_po,
+                                          rice_limit, est.ctypes.data))
+    return est
+
+
+def debug_lpc(autoc, meta, cands, max_order, qlp_precision, prec_search, exhaustive, blocksize, autoc_unshifted=False, device=0):
+    """Test hook fb200_debug_lpc: the encoder's LPC analysis kernel on given autocorrelations.
+    autoc: float64 [nsec, nitems, lag_stride]; meta: int [nitems, 2] (wasted bits, subframe bps); cands: int [nwin, 3] (kind, sec,
+    root). Returns int32 [nitems, nwin * slots per window, 40]: each slot's CandDesc fields in order (valid, order, precision,
+    shift, wide, limit, two pad words, qlp[32])."""
+    a = np.ascontiguousarray(autoc, dtype=np.float64)
+    m = np.ascontiguousarray(meta, dtype=np.int32).reshape(-1, 2)
+    c = np.ascontiguousarray(cands, dtype=np.int32).reshape(-1, 3)
+    nsec, nitems, lag_stride = a.shape
+    assert m.shape[0] == nitems
+    per_item = c.shape[0] * (max_order if exhaustive else 1) * (15 - 5 + 1 if prec_search else 1)
+    out = (CandDesc * (nitems * per_item))()
+    nslots = C.c_uint32(0)
+    _check(lib().fb200_debug_lpc(device, a.ctypes.data, nsec, lag_stride, m.ctypes.data, c.ctypes.data, c.shape[0], nitems, max_order,
+                                 qlp_precision, int(prec_search), int(exhaustive), blocksize, int(autoc_unshifted), out,
+                                 C.sizeof(CandDesc), C.byref(nslots)))
+    assert nslots.value == per_item
+    return np.frombuffer(out, dtype=np.int32).reshape(nitems, per_item, C.sizeof(CandDesc) // 4).copy()
 
 
 def debug_replaygain_windows(d_pcm_ptr, pcm_values, files, capacity, device=0, stream=0):

@@ -1663,6 +1663,119 @@ int fb200_debug_log(const double *x, double *y, uint32_t n, int device)
 	return FB200_OK;
 }
 
+// k_lpc on caller-supplied autocorrelations (tests/test_gpu_lpc_edges.py), launched by launch_lpc as the encoder launches it
+int fb200_debug_lpc(int device, const double *autoc, uint32_t nsec, uint32_t lag_stride, const int32_t *meta, const int32_t *cands,
+                    uint32_t nwin, uint32_t nitems, uint32_t max_order, uint32_t qlp_precision, int prec_search, int exhaustive,
+                    uint32_t blocksize, int autoc_unshifted, void *out, size_t cand_bytes, uint32_t *nslots_out)
+{
+	if(!autoc || !meta || !cands || !out || !nslots_out) return FB200_ERR_INVALID;
+	if(cand_bytes != sizeof(CandDesc)) { set_error("candidate size mismatch %zu != %zu", cand_bytes, sizeof(CandDesc)); return FB200_ERR_INVALID; }
+	if(max_order < 1 || max_order > FB200_MAX_LPC_ORDER || max_order >= blocksize || blocksize > 65535 || lag_stride < max_order + 1 ||
+	   nsec == 0 || nwin == 0 || nitems == 0 || (!prec_search && (qlp_precision < kMinQlpPrecision || qlp_precision > kMaxQlpPrecision))) {
+		set_error("fb200_debug_lpc: arguments out of range");
+		return FB200_ERR_INVALID;
+	}
+	for(uint32_t i = 0; i < nitems; i++)
+		if(meta[2 * i] < 0 || meta[2 * i] > 31 || meta[2 * i + 1] < 0 || meta[2 * i + 1] > 32) { set_error("fb200_debug_lpc: meta %u", i); return FB200_ERR_INVALID; }
+	for(uint32_t w = 0; w < nwin; w++) {
+		const int32_t *c = cands + 3 * w;
+		if(c[0] < 0 || c[0] > 1 || c[1] < 0 || (uint32_t)c[1] >= nsec || c[2] < 0 || (uint32_t)c[2] >= nsec) { set_error("fb200_debug_lpc: candidate %u", w); return FB200_ERR_INVALID; }
+	}
+	EncK k;
+	memset(&k, 0, sizeof k);
+	k.bs = (int)blocksize;
+	k.max_order = (int)max_order;
+	k.lags = k.max_order + 1;
+	k.lag_stride = (int)lag_stride;
+	k.qlp_precision = (int)qlp_precision;
+	k.prec_search = prec_search ? 1 : 0;
+	k.exhaustive = exhaustive ? 1 : 0;
+	k.nsec = (int)nsec;
+	k.nwin = (int)nwin;
+	k.nslots = k.nwin * (k.exhaustive ? k.max_order : 1) * (k.prec_search ? kQlpPrecisionSteps : 1);  // as the encoder sizes them
+	*nslots_out = (uint32_t)k.nslots;
+	const size_t nac = (size_t)nsec * nitems * lag_stride, nout = (size_t)nitems * k.nslots;
+	std::vector<DevCand> hc(nwin);
+	for(uint32_t w = 0; w < nwin; w++) hc[w] = DevCand{cands[3 * w], cands[3 * w + 1], cands[3 * w + 2]};
+	std::vector<SigMeta> hm(nitems);
+	for(uint32_t i = 0; i < nitems; i++) hm[i] = SigMeta{meta[2 * i], meta[2 * i + 1]};
+	FB_CUDA(cudaSetDevice(device));
+	double *d_ac = nullptr;
+	DevCand *d_c = nullptr;
+	SigMeta *d_m = nullptr;
+	CandDesc *d_o = nullptr;
+	int rc = FB200_OK;
+	if(cudaMalloc(&d_ac, nac * sizeof(double)) != cudaSuccess || cudaMalloc(&d_c, nwin * sizeof(DevCand)) != cudaSuccess ||
+	   cudaMalloc(&d_m, nitems * sizeof(SigMeta)) != cudaSuccess || cudaMalloc(&d_o, nout * sizeof(CandDesc)) != cudaSuccess ||
+	   cudaMemcpy(d_ac, autoc, nac * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
+	   cudaMemcpy(d_c, hc.data(), nwin * sizeof(DevCand), cudaMemcpyHostToDevice) != cudaSuccess ||
+	   cudaMemcpy(d_m, hm.data(), nitems * sizeof(SigMeta), cudaMemcpyHostToDevice) != cudaSuccess ||
+	   cudaMemset(d_o, 0xff, nout * sizeof(CandDesc)) != cudaSuccess) {
+		set_error("fb200_debug_lpc: %s", cudaGetErrorString(cudaGetLastError()));
+		rc = FB200_ERR_CUDA;
+	}
+	if(rc == FB200_OK) {
+		launch_lpc(k, d_ac, d_c, d_m, nullptr, d_o, (int)nitems, autoc_unshifted ? 1 : 0, 0);
+		cudaError_t err = cudaGetLastError();
+		if(err == cudaSuccess) err = cudaMemcpy(out, d_o, nout * sizeof(CandDesc), cudaMemcpyDeviceToHost);
+		if(err != cudaSuccess) { set_error("fb200_debug_lpc: %s", cudaGetErrorString(err)); rc = FB200_ERR_CUDA; }
+	}
+	cudaFree(d_ac); cudaFree(d_c); cudaFree(d_m); cudaFree(d_o);
+	return rc;
+}
+
+// the general search kernel's evaluation of given LPC candidates on given signals (tests/test_gpu_lpc_edges.py)
+int fb200_debug_evaluate_lpc(int device, const int32_t *signals, const int32_t *meta, const void *cands, size_t cand_bytes, uint32_t n,
+                             uint32_t blocksize, uint32_t min_po, uint32_t max_po, uint32_t rice_limit, uint32_t *est)
+{
+	if(!signals || !meta || !cands || !est || n == 0) return FB200_ERR_INVALID;
+	if(cand_bytes != sizeof(CandDesc)) { set_error("candidate size mismatch %zu != %zu", cand_bytes, sizeof(CandDesc)); return FB200_ERR_INVALID; }
+	if(blocksize < 16 || blocksize > 65535 || max_po > (uint32_t)kMaxPartitionOrder || min_po > max_po || (rice_limit != 15 && rice_limit != 31)) {
+		set_error("fb200_debug_evaluate_lpc: arguments out of range");
+		return FB200_ERR_INVALID;
+	}
+	const CandDesc *hc = static_cast<const CandDesc *>(cands);
+	std::vector<SigMeta> hm(n);
+	for(uint32_t i = 0; i < n; i++) {
+		hm[i] = SigMeta{meta[2 * i], meta[2 * i + 1]};
+		if(hm[i].wasted < 0 || hm[i].wasted > 31 || hm[i].bps < 1 || hm[i].bps > 32 || hc[i].order < 1 || hc[i].order > FB200_MAX_LPC_ORDER ||
+		   (uint32_t)hc[i].order >= blocksize || hc[i].shift < 0 || hc[i].shift > 15) {
+			set_error("fb200_debug_evaluate_lpc: candidate %u", i);
+			return FB200_ERR_INVALID;
+		}
+	}
+	EncK k;
+	memset(&k, 0, sizeof k);
+	k.bs = k.bs_stride = (int)blocksize;
+	k.min_po = (int)min_po;
+	k.max_po = (int)max_po;
+	k.rice_limit = (int)rice_limit;
+	FB_CUDA(cudaSetDevice(device));
+	const size_t ns = (size_t)n * blocksize;
+	int32_t *d_sig = nullptr;
+	SigMeta *d_m = nullptr;
+	CandDesc *d_c = nullptr;
+	uint32_t *d_absr = nullptr, *d_est = nullptr;
+	int rc = FB200_OK;
+	if(cudaMalloc(&d_sig, ns * sizeof(int32_t)) != cudaSuccess || cudaMalloc(&d_m, n * sizeof(SigMeta)) != cudaSuccess ||
+	   cudaMalloc(&d_c, n * sizeof(CandDesc)) != cudaSuccess || cudaMalloc(&d_absr, ns * sizeof(uint32_t)) != cudaSuccess ||
+	   cudaMalloc(&d_est, n * sizeof(uint32_t)) != cudaSuccess ||
+	   cudaMemcpy(d_sig, signals, ns * sizeof(int32_t), cudaMemcpyHostToDevice) != cudaSuccess ||
+	   cudaMemcpy(d_m, hm.data(), n * sizeof(SigMeta), cudaMemcpyHostToDevice) != cudaSuccess ||
+	   cudaMemcpy(d_c, hc, n * sizeof(CandDesc), cudaMemcpyHostToDevice) != cudaSuccess) {
+		set_error("fb200_debug_evaluate_lpc: %s", cudaGetErrorString(cudaGetLastError()));
+		rc = FB200_ERR_CUDA;
+	}
+	if(rc == FB200_OK) {
+		launch_debug_evaluate(k, d_sig, d_m, d_c, d_absr, d_est, (int)n);
+		cudaError_t err = cudaGetLastError();
+		if(err == cudaSuccess) err = cudaMemcpy(est, d_est, n * sizeof(uint32_t), cudaMemcpyDeviceToHost);
+		if(err != cudaSuccess) { set_error("fb200_debug_evaluate_lpc: %s", cudaGetErrorString(err)); rc = FB200_ERR_CUDA; }
+	}
+	cudaFree(d_sig); cudaFree(d_m); cudaFree(d_c); cudaFree(d_absr); cudaFree(d_est);
+	return rc;
+}
+
 // ---- debug/stage-level access for the parity tests (plans of the last launch) ----
 int fb200_debug_copy_plans(fb200_encoder *e, uint32_t nblocks, void *host_plans, size_t plan_bytes, uint32_t *host_chan_assign)
 {

@@ -177,6 +177,7 @@ void launch_meta(const EncK &k, const int32_t *pcm, SigMeta *meta, int *blkflags
 void launch_prep(const EncK &k, const int32_t *pcm, int32_t *sig, SigMeta *meta, int *blkflags, int nb, cudaStream_t st);
 void launch_autoc_general(const EncK &k, const int32_t *sig, const SigMeta *meta, const float *windows, const DevSection *secs, double *autoc, int nitems, cudaStream_t st);
 void launch_minbr_flags(const EncK &k, const SubframePlan *plans, const int *blkflags, int nb, int *flags, cudaStream_t st);
+void launch_debug_evaluate(const EncK &k, const int32_t *sig, const SigMeta *meta, const CandDesc *cands, uint32_t *absr, uint32_t *est, int n);
 void launch_lpc(const EncK &k, const double *autoc, const DevCand *cands, SigMeta *meta, const uint32_t *sigor, CandDesc *cdesc, int nitems, int autoc_unshifted, cudaStream_t st);
 void launch_search_general(const EncK &k, size_t smem, const int32_t *sig, const SigMeta *meta, const CandDesc *cdesc, SubframePlan *plans, int nitems, cudaStream_t st);
 void launch_emit_general(const EncK &k, size_t smem, const int32_t *sig, const int *blkflags, const SubframePlan *plans, uint8_t *slots, uint32_t *frame_bytes, uint32_t *chan_assign, int nb, cudaStream_t st);

@@ -71,6 +71,27 @@ void launch_gather(const EncK &k, const uint8_t *slots, const uint32_t *bytes, c
 	k_gather<<<nb, 256, 0, st>>>(k, slots, bytes, offsets, out, capacity, err);
 }
 
+// fb200_debug_evaluate_lpc: evaluate_candidate (k_search's per-candidate evaluation) on one LPC candidate per CTA; est = its
+// estimate, 0xffffffff when the candidate is rejected
+__global__ void __launch_bounds__(128) k_debug_evaluate(EncK P, const int32_t *__restrict__ sig, const SigMeta *__restrict__ meta,
+                                                        const CandDesc *__restrict__ cands, uint32_t *__restrict__ absr, uint32_t *__restrict__ est)
+{
+	__shared__ SearchShared S;
+	const int c = blockIdx.x;
+	if(threadIdx.x == 0) { S.fail = 0; S.best_bits = 0xffffffffu; }
+	if(threadIdx.x < FB200_MAX_LPC_ORDER) S.c_qlp[threadIdx.x] = cands[c].qlp[threadIdx.x];
+	__syncthreads();
+	const CandDesc &D = cands[c];
+	evaluate_candidate(P, S, sig + (size_t)c * P.bs, absr + (size_t)c * P.bs, SF_LPC, D.order, D.precision, D.shift, D.wide, D.limit,
+	                   meta[c].bps, meta[c].wasted);
+	if(threadIdx.x == 0) est[c] = S.best_bits;
+}
+
+void launch_debug_evaluate(const EncK &k, const int32_t *sig, const SigMeta *meta, const CandDesc *cands, uint32_t *absr, uint32_t *est, int n)
+{
+	k_debug_evaluate<<<n, 128>>>(k, sig, meta, cands, absr, est);
+}
+
 void launch_debug_log(const double *dx, double *dy, int n) { k_debug_log<<<(n + 255) / 256, 256>>>(dx, dy, n); }
 
 // The dynamic shared-memory opt-in is a per-function, per-device attribute: set it ONCE to the device maximum, so that

@@ -566,6 +566,22 @@ int fb200_debug_copy_plans(fb200_encoder *enc, uint32_t nblocks, void *host_plan
 int fb200_debug_perturb_verify(fb200_encoder *enc, uint32_t file, uint32_t what, uint32_t a, uint32_t b, uint32_t xor_mask);
 /* y[i] = the engine's device restatement of the host libm's log(x[i]) (reference: lpc.c:1594, fixed.c:284). */
 int fb200_debug_log(const double *x, double *y, uint32_t n, int device);
+/* The encoder's LPC analysis kernel (Levinson-Durbin, order guess, precision loop, quantisation, residual-width flags) on
+ * caller-supplied autocorrelations, with the kernel instantiation the encoder takes for max_order (8, 12 or 32).
+ * autoc: nsec x nitems records of lag_stride doubles, record (sec, item) at (sec * nitems + item) * lag_stride, entries
+ * [0 .. max_order] used. meta: per item (wasted bits, subframe bps). cands: per window (kind, sec, root); kind 1 is a punch-out
+ * window, autoc[sec, root][l] - autoc[sec][l] for l < max_order. autoc_unshifted: the records are of the signal before its
+ * wasted bits were shifted out. out: nitems x *nslots_out records of cand_bytes (fb200::CandDesc,
+ * flac_b200/csrc/fb200_internal.h), window w's slots from w * (*nslots_out / nwin). */
+/* The general search kernel's evaluation of one LPC candidate (residual -- 32-bit, 64-bit or checked as its wide / limit flags
+ * say --, partition sums, Rice parameters, bit estimate) on each of n signals of blocksize samples: signal i is
+ * signals[i * blocksize ..], meta[i] its (wasted bits, subframe bps), cands[i] an fb200::CandDesc (cand_bytes each). est[i] is
+ * the estimate, 0xffffffff when the candidate is rejected (a checked residual outside int32). */
+int fb200_debug_evaluate_lpc(int device, const int32_t *signals, const int32_t *meta, const void *cands, size_t cand_bytes, uint32_t n,
+                             uint32_t blocksize, uint32_t min_po, uint32_t max_po, uint32_t rice_limit, uint32_t *est);
+int fb200_debug_lpc(int device, const double *autoc, uint32_t nsec, uint32_t lag_stride, const int32_t *meta, const int32_t *cands,
+                    uint32_t nwin, uint32_t nitems, uint32_t max_order, uint32_t qlp_precision, int prec_search, int exhaustive,
+                    uint32_t blocksize, int autoc_unshifted, void *out, size_t cand_bytes, uint32_t *nslots_out);
 
 /* ---- decoder ----
  * Batch frame decode (read_frame_ for many frames). The caller supplies frame boundaries

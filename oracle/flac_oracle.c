@@ -53,6 +53,7 @@ struct fo_encoder {
 	int32_t *residual;
 	float *windowed;
 	uint64_t *psums;
+	fo_lpc_cand lpc_cands[FO_MAX_LPC_CANDIDATES];  /* one apodization's candidates */
 };
 
 /* ------------------------------------------------------------------ bit math */
@@ -72,6 +73,16 @@ static uint32_t silog2(int64_t v)
 	if(v == -1) return 2;
 	v = (v < 0) ? (-(v + 1)) : v;
 	return ilog2_64((uint64_t)v) + 2;
+}
+
+uint32_t fo_silog2(int64_t v) { return silog2(v); }
+
+static fo_lpc_counters counters;
+
+void fo_lpc_counters_get(fo_lpc_counters *out, int reset)
+{
+	if(out) *out = counters;
+	if(reset) memset(&counters, 0, sizeof counters);
 }
 
 /* ------------------------------------------------------------------ CRC (crc.c:39-396) */
@@ -453,6 +464,7 @@ void fo_lp_coefficients(const double *autoc, uint32_t *max_order, float lp_coeff
 		error[i] = err;
 
 		if(err == 0.0) {
+			if(i + 1 < *max_order) counters.levinson_early++;
 			*max_order = i + 1;
 			return;
 		}
@@ -514,8 +526,10 @@ int fo_quantize_coefficients(const float *lp_coeff, uint32_t order, uint32_t pre
 		const double d = fabs(lp_coeff[i]);
 		if(d > cmax) cmax = d;
 	}
-	if(cmax <= 0.0)
+	if(cmax <= 0.0) {
+		counters.cmax_zero++;
 		return 2;
+	}
 	else {
 		const int max_shiftlimit = (1 << (LPC_QLP_SHIFT_LEN - 1)) - 1;
 		const int min_shiftlimit = -max_shiftlimit - 1;
@@ -523,10 +537,14 @@ int fo_quantize_coefficients(const float *lp_coeff, uint32_t order, uint32_t pre
 		(void)frexp(cmax, &log2cmax);
 		log2cmax--;
 		*shift = (int)precision - log2cmax - 1;
-		if(*shift > max_shiftlimit)
+		if(*shift > max_shiftlimit) {
 			*shift = max_shiftlimit;
-		else if(*shift < min_shiftlimit)
+			counters.shift_clamped++;
+		}
+		else if(*shift < min_shiftlimit) {
+			counters.shift_too_small++;
 			return 1;
+		}
 	}
 
 	if(*shift >= 0) {
@@ -534,7 +552,9 @@ int fo_quantize_coefficients(const float *lp_coeff, uint32_t order, uint32_t pre
 		int32_t q;
 		for(i = 0; i < order; i++) {
 			error += lp_coeff[i] * (1 << *shift);   /* float * int -> float product, then double add */
+			if(fabs(error - trunc(error)) == 0.5) counters.round_half++;
 			q = (int32_t)lround(error);
+			if(q > qmax || q < qmin) counters.coef_clipped++;
 			if(q > qmax) q = qmax;
 			else if(q < qmin) q = qmin;
 			error -= q;
@@ -544,10 +564,13 @@ int fo_quantize_coefficients(const float *lp_coeff, uint32_t order, uint32_t pre
 	else {
 		const int nshift = -(*shift);
 		double error = 0.0;
+		counters.negative_shift++;
 		int32_t q;
 		for(i = 0; i < order; i++) {
 			error += lp_coeff[i] / (1 << nshift);
+			if(fabs(error - trunc(error)) == 0.5) counters.round_half++;
 			q = (int32_t)lround(error);
+			if(q > qmax || q < qmin) counters.coef_clipped++;
 			if(q > qmax) q = qmax;
 			else if(q < qmin) q = qmin;
 			error -= q;
@@ -559,7 +582,7 @@ int fo_quantize_coefficients(const float *lp_coeff, uint32_t order, uint32_t pre
 }
 
 /* lpc.c:942-968 */
-static uint64_t max_prediction_value_before_shift(uint32_t subframe_bps, const int32_t *qlp, uint32_t order)
+uint64_t fo_max_prediction_value_before_shift(uint32_t subframe_bps, const int32_t *qlp, uint32_t order)
 {
 	uint64_t max_abs_sample_value = (uint64_t)1 << (subframe_bps - 1);
 	uint32_t abs_sum = 0, i;
@@ -568,10 +591,10 @@ static uint64_t max_prediction_value_before_shift(uint32_t subframe_bps, const i
 	return max_abs_sample_value * abs_sum;
 }
 
-static uint32_t max_residual_bps(uint32_t subframe_bps, const int32_t *qlp, uint32_t order, int lp_quantization)
+uint32_t fo_max_residual_bps(uint32_t subframe_bps, const int32_t *qlp, uint32_t order, int lp_quantization)
 {
 	uint64_t max_abs_sample_value = (uint64_t)1 << (subframe_bps - 1);
-	uint64_t max_pred_after = (uint64_t)(-1 * ((-1 * (int64_t)max_prediction_value_before_shift(subframe_bps, qlp, order)) >> lp_quantization));
+	uint64_t max_pred_after = (uint64_t)(-1 * ((-1 * (int64_t)fo_max_prediction_value_before_shift(subframe_bps, qlp, order)) >> lp_quantization));
 	uint64_t max_residual_value = max_abs_sample_value + max_pred_after;
 	return silog2((int64_t)max_residual_value);
 }
@@ -756,6 +779,7 @@ static uint32_t find_best_partition_order(fo_encoder *e, const int32_t *residual
 				const int32_t r = residual[rs];
 				s += (uint32_t)(r < 0 ? -(uint32_t)r : (uint32_t)r);
 			}
+			if(narrow && s > UINT32_MAX) counters.narrow_wrapped++;
 			sums[partition] = narrow ? (uint64_t)(uint32_t)s : s;
 		}
 		to = partitions;
@@ -823,32 +847,32 @@ static uint32_t evaluate_fixed(fo_encoder *e, const int32_t *signal, uint32_t bl
 	return estimate;
 }
 
-/* stream_encoder.c:4564-4666 evaluate_lpc_subframe_ */
-static uint32_t evaluate_lpc(fo_encoder *e, const int32_t *signal, const float *lp_coeff, uint32_t blocksize, uint32_t subframe_bps, uint32_t wasted,
-                             uint32_t order, uint32_t qlp_coeff_precision, uint32_t rice_limit, uint32_t min_po, uint32_t max_po, fo_subframe_plan *plan)
+/* stream_encoder.c:4564-4666 evaluate_lpc_subframe_, from :4600 on (the candidate was quantised by fo_lpc_candidates) */
+static uint32_t evaluate_lpc(fo_encoder *e, const int32_t *signal, const fo_lpc_cand *c, uint32_t blocksize, uint32_t subframe_bps, uint32_t wasted,
+                             uint32_t rice_limit, uint32_t min_po, uint32_t max_po, fo_subframe_plan *plan)
 {
-	int32_t qlp[FO_MAX_LPC_ORDER];
+	const uint32_t order = (uint32_t)c->order, qlp_coeff_precision = (uint32_t)c->precision;
+	const int32_t *qlp = c->qlp;
+	const int quantization = c->shift;
 	const uint32_t residual_samples = blocksize - order;
 	uint32_t residual_bits, estimate;
-	int quantization, limit;
+	int limit;
 
-	if(subframe_bps <= 17)
-		qlp_coeff_precision = MINU(qlp_coeff_precision, 32 - subframe_bps - ilog2_64(order));
-
-	memset(qlp, 0, sizeof qlp);
-	if(fo_quantize_coefficients(lp_coeff, order, qlp_coeff_precision, qlp, &quantization) != 0)
+	limit = fo_max_residual_bps(subframe_bps, qlp, order, quantization) > 32;
+	if(limit) counters.limit++;
+	if(limit || silog2((int64_t)fo_max_prediction_value_before_shift(subframe_bps, qlp, order)) > 32) counters.wide++;
+	if(!lpc_residual(signal + order, residual_samples, qlp, order, quantization, e->residual, limit)) {
+		counters.limit_rejected++;
 		return 0;
-
-	limit = max_residual_bps(subframe_bps, qlp, order, quantization) > 32;
-	if(!lpc_residual(signal + order, residual_samples, qlp, order, quantization, e->residual, limit))
-		return 0;
+	}
 
 	plan_reset(plan, wasted, subframe_bps);
 	plan->type = 3;
 	plan->order = (int32_t)order;
 	plan->qlp_precision = (int32_t)qlp_coeff_precision;
 	plan->qlp_shift = quantization;
-	memcpy(plan->qlp_coeff, qlp, sizeof qlp);
+	plan->qlp_negative_shift = c->negative_shift;
+	memcpy(plan->qlp_coeff, qlp, sizeof plan->qlp_coeff);
 	residual_bits = find_best_partition_order(e, e->residual, residual_samples, order, rice_limit, min_po, max_po, subframe_bps, plan);
 
 	estimate = SUBFRAME_HEADER_BITS + wasted + LPC_QLP_PRECISION_LEN + LPC_QLP_SHIFT_LEN + order * (qlp_coeff_precision + subframe_bps);
@@ -856,6 +880,15 @@ static uint32_t evaluate_lpc(fo_encoder *e, const int32_t *signal, const float *
 	else estimate = UINT32_MAX;
 	plan->estimate_bits = estimate;
 	return estimate;
+}
+
+uint32_t fo_lpc_estimate(fo_encoder *e, const int32_t *signal, uint32_t blocksize, uint32_t subframe_bps, uint32_t wasted,
+                         const fo_lpc_cand *c, uint32_t min_po, uint32_t max_po)
+{
+	fo_subframe_plan plan;
+	if(blocksize > e->cfg.blocksize || c->order < 1 || (uint32_t)c->order >= blocksize) return 0;
+	return evaluate_lpc(e, signal, c, blocksize, subframe_bps, wasted, e->cfg.bits_per_sample > 16 ? RICE2_ESCAPE : RICE_ESCAPE, min_po,
+	                    max_po, &plan);
 }
 
 /* stream_encoder.c:4293-4316 set_next_subdivide_tukey */
@@ -880,17 +913,16 @@ typedef struct {
  * autoc_root copies only max_order entries (:4340) and the punch-out subtraction covers
  * only max_order entries (:4370-4371), so autoc[max_order] keeps the preceding partial
  * window's value. */
-static int apply_apodization(fo_encoder *e, apod_state *st, uint32_t blocksize, double *lpc_error, uint32_t *max_order_this, uint32_t subframe_bps,
-                             const int32_t *signal, float lp_coeff[][FO_MAX_LPC_ORDER], uint32_t *guess_lpc_order)
+static int apply_apodization(fo_encoder *e, apod_state *st, uint32_t blocksize, uint32_t max_order, const int32_t *signal)
 {
 	const fo_apodization *cur = &e->cfg.apodizations[st->a];
 	const float *win = e->window[st->a];
 
 	if(st->b == 1) {
 		window_data(signal, win, e->windowed, blocksize);
-		fo_autocorrelation(e->windowed, blocksize, (*max_order_this) + 1, st->autoc);
+		fo_autocorrelation(e->windowed, blocksize, max_order + 1, st->autoc);
 		if(cur->type == FO_APOD_SUBDIVIDE_TUKEY) {
-			memcpy(st->autoc_root, st->autoc, *max_order_this * sizeof(st->autoc[0]));
+			memcpy(st->autoc_root, st->autoc, max_order * sizeof(st->autoc[0]));
 			st->b++;
 		}
 		else
@@ -903,22 +935,74 @@ static int apply_apodization(fo_encoder *e, apod_state *st, uint32_t blocksize, 
 		}
 		if(!(st->c % 2)) {
 			window_data_partial(signal, win, e->windowed, blocksize, blocksize / st->b / 2, (st->c / 2 * blocksize) / st->b);
-			fo_autocorrelation(e->windowed, blocksize / st->b, (*max_order_this) + 1, st->autoc);
+			fo_autocorrelation(e->windowed, blocksize / st->b, max_order + 1, st->autoc);
 		}
 		else {
 			uint32_t i;
-			for(i = 0; i < *max_order_this; i++)
+			for(i = 0; i < max_order; i++)
 				st->autoc[i] = st->autoc_root[i] - st->autoc[i];
 		}
 		next_subdivide_tukey(cur->parts, &st->a, &st->b, &st->c);
 	}
-
-	if(st->autoc[0] == 0.0)
-		return 0;
-	fo_lp_coefficients(st->autoc, max_order_this, lp_coeff, lpc_error);
-	*guess_lpc_order = fo_best_order(lpc_error, *max_order_this, blocksize,
-	                                 subframe_bps + (e->cfg.do_qlp_coeff_prec_search ? MIN_QLP_PRECISION : e->cfg.qlp_coeff_precision));
 	return 1;
+}
+
+/* stream_encoder.c:4376-4391 (the tail of apply_apodization_) and :4220-4260 + 4591-4599 (process_subframe_'s order and
+ * precision loops, and the start of evaluate_lpc_subframe_ up to the quantisation) */
+size_t fo_lpc_candidates(const double *autoc, uint32_t max_order, uint32_t subframe_bps, uint32_t blocksize, const fo_config *cfg,
+                         fo_lpc_cand *out)
+{
+	float lp_coeff[FO_MAX_LPC_ORDER][FO_MAX_LPC_ORDER];
+	double lpc_error[FO_MAX_LPC_ORDER];
+	uint32_t min_lpc, lo, guess;
+	size_t n = 0;
+
+	if(autoc[0] == 0.0)
+		return 0;
+	fo_lp_coefficients(autoc, &max_order, lp_coeff, lpc_error);
+	guess = fo_best_order(lpc_error, max_order, blocksize,
+	                      subframe_bps + (cfg->do_qlp_coeff_prec_search ? MIN_QLP_PRECISION : cfg->qlp_coeff_precision));
+	if(cfg->do_exhaustive_model_search) min_lpc = 1;
+	else min_lpc = max_order = guess;
+	for(lo = min_lpc; lo <= max_order; lo++) {
+		uint32_t minp, maxp, prec;
+		double lbps = expected_bits(lpc_error[lo - 1], blocksize - lo);
+		if(lbps >= (double)subframe_bps) {
+			counters.order_skipped++;
+			memset(&out[n], 0, sizeof out[n]);
+			out[n].status = FO_LPC_DONT_EVEN_TRY;
+			out[n++].order = (int32_t)lo;
+			continue;
+		}
+		if(cfg->do_qlp_coeff_prec_search) {
+			minp = MIN_QLP_PRECISION;
+			if(subframe_bps <= 17) {
+				maxp = MINU(32 - subframe_bps - ilog2_64(lo), MAX_QLP_PRECISION);
+				maxp = MAXU(maxp, minp);
+			}
+			else maxp = MAX_QLP_PRECISION;
+		}
+		else minp = maxp = cfg->qlp_coeff_precision;
+		for(prec = minp; prec <= maxp; prec++) {
+			fo_lpc_cand *c = &out[n++];
+			uint32_t precision = prec;
+			memset(c, 0, sizeof *c);
+			if(subframe_bps <= 17 && 32 - subframe_bps - ilog2_64(lo) < precision) {
+				precision = 32 - subframe_bps - ilog2_64(lo);
+				counters.precision_capped++;
+			}
+			c->order = (int32_t)lo;
+			c->precision_tried = (int32_t)prec;
+			c->precision = (int32_t)precision;
+			{
+				const uint64_t neg = counters.negative_shift;
+				c->status = fo_quantize_coefficients(lp_coeff[lo - 1], lo, precision, c->qlp, &c->shift);
+				c->negative_shift = counters.negative_shift != neg;
+			}
+			if(c->status != FO_LPC_QUANTIZED) c->shift = 0;
+		}
+	}
+	return n;
 }
 
 /* stream_encoder.c:4045-4290 process_subframe_: best-of-two search in evaluation order
@@ -980,34 +1064,18 @@ static uint32_t process_subframe(fo_encoder *e, const int32_t *signal, uint32_t 
 				uint32_t max_lpc_order = cfg->max_lpc_order >= blocksize ? blocksize - 1 : cfg->max_lpc_order;
 				if(max_lpc_order > 0) {
 					apod_state st;
-					float lp_coeff[FO_MAX_LPC_ORDER][FO_MAX_LPC_ORDER];
-					double lpc_error[FO_MAX_LPC_ORDER];
 					memset(&st, 0, sizeof st);
 					st.a = 0; st.b = 1; st.c = 0;
 					while(st.a < cfg->num_apodizations) {
-						uint32_t max_this = max_lpc_order, min_lpc, guess = 0, lo;
-						if(!apply_apodization(e, &st, blocksize, lpc_error, &max_this, subframe_bps, signal, lp_coeff, &guess))
+						size_t n, i;
+						if(!apply_apodization(e, &st, blocksize, max_lpc_order, signal))
 							continue;
-						if(cfg->do_exhaustive_model_search) min_lpc = 1;
-						else min_lpc = max_this = guess;
-						for(lo = min_lpc; lo <= max_this; lo++) {
-							uint32_t minp, maxp, prec;
-							double lbps = expected_bits(lpc_error[lo - 1], blocksize - lo);
-							if(lbps >= (double)subframe_bps)
+						n = fo_lpc_candidates(st.autoc, max_lpc_order, subframe_bps, blocksize, cfg, e->lpc_cands);
+						for(i = 0; i < n; i++) {
+							if(e->lpc_cands[i].status != FO_LPC_QUANTIZED)
 								continue;
-							if(cfg->do_qlp_coeff_prec_search) {
-								minp = MIN_QLP_PRECISION;
-								if(subframe_bps <= 17) {
-									maxp = MINU(32 - subframe_bps - ilog2_64(lo), MAX_QLP_PRECISION);
-									maxp = MAXU(maxp, minp);
-								}
-								else maxp = MAX_QLP_PRECISION;
-							}
-							else minp = maxp = cfg->qlp_coeff_precision;
-							for(prec = minp; prec <= maxp; prec++) {
-								cand_bits = evaluate_lpc(e, signal, lp_coeff[lo - 1], blocksize, subframe_bps, wasted, lo, prec, rice_limit, min_po, max_po, &cand);
-								if(cand_bits > 0 && cand_bits < best_bits) { *best = cand; best_bits = cand_bits; }
-							}
+							cand_bits = evaluate_lpc(e, signal, &e->lpc_cands[i], blocksize, subframe_bps, wasted, rice_limit, min_po, max_po, &cand);
+							if(cand_bits > 0 && cand_bits < best_bits) { *best = cand; best_bits = cand_bits; }
 						}
 					}
 				}

@@ -69,6 +69,7 @@ typedef struct {
 	int32_t wasted_bits;
 	int32_t subframe_bps;
 	int32_t qlp_precision, qlp_shift;
+	int32_t qlp_negative_shift; /* lpc: quantised through the divide branch (computed shift < 0, coded as 0) */
 	int32_t qlp_coeff[FO_MAX_LPC_ORDER];
 	int32_t rice_method;     /* 0 RICE, 1 RICE2 */
 	int32_t partition_order;
@@ -115,6 +116,56 @@ uint32_t fo_best_order(const double *lpc_error, uint32_t max_order, uint32_t tot
 int fo_quantize_coefficients(const float *lp_coeff, uint32_t order, uint32_t precision, int32_t *qlp_coeff, int *shift);
 uint8_t fo_crc8(const uint8_t *data, size_t len);
 uint16_t fo_crc16(const uint8_t *data, size_t len);
+/* lpc.c:942-968 FLAC__lpc_max_prediction_value_before_shift / FLAC__lpc_max_residual_bps */
+uint64_t fo_max_prediction_value_before_shift(uint32_t subframe_bps, const int32_t *qlp, uint32_t order);
+uint32_t fo_max_residual_bps(uint32_t subframe_bps, const int32_t *qlp, uint32_t order, int lp_quantization);
+uint32_t fo_silog2(int64_t v);
+
+/* One LPC candidate of one apodization, in the order process_subframe_ evaluates them (stream_encoder.c:4220-4260, 4591-4599). */
+enum { FO_LPC_QUANTIZED = 0, FO_LPC_SHIFT_TOO_SMALL = 1, FO_LPC_CMAX_ZERO = 2, FO_LPC_DONT_EVEN_TRY = 3 };
+typedef struct {
+	int32_t status;          /* FO_LPC_*: 1 and 2 are quantize_coefficients' return codes; 3 skips the whole order */
+	int32_t order;
+	int32_t precision_tried; /* the precision the search asked for */
+	int32_t precision;       /* after the <= 17-bit cap */
+	int32_t shift;
+	int32_t negative_shift;  /* quantised through the divide branch: the computed shift was negative, the coded one is 0 */
+	int32_t qlp[FO_MAX_LPC_ORDER];
+} fo_lpc_cand;
+#define FO_MAX_LPC_CANDIDATES (FO_MAX_LPC_ORDER * (15 - 5 + 1))
+
+/* Levinson-Durbin on autoc[0 .. max_order], the order guess (or every order with do_exhaustive_model_search) and every
+ * precision the configuration tries (cfg: do_qlp_coeff_prec_search, qlp_coeff_precision, do_exhaustive_model_search).
+ * Returns the number of candidates written to out (at most FO_MAX_LPC_CANDIDATES); 0 when autoc[0] == 0. The frame encoder
+ * evaluates exactly these. */
+size_t fo_lpc_candidates(const double *autoc, uint32_t max_order, uint32_t subframe_bps, uint32_t blocksize, const fo_config *cfg,
+                         fo_lpc_cand *out);
+
+/* evaluate_lpc_subframe_ from the residual on (stream_encoder.c:4600-4666) for one quantised candidate on one subframe, with
+ * the encoder's Rice parameter limit and the given partition orders: the estimate, 0 when a checked residual leaves int32. */
+uint32_t fo_lpc_estimate(fo_encoder *e, const int32_t *signal, uint32_t blocksize, uint32_t subframe_bps, uint32_t wasted,
+                         const fo_lpc_cand *c, uint32_t min_po, uint32_t max_po);
+
+/* How often the encoder took each rarely reached branch of its LPC stage, summed over every call in the process since the
+ * last reset. The counters are one process-wide static that every encode increments without synchronisation: encodes run
+ * concurrently from several threads race on them (their frames stay correct, the counts do not), so read them only from
+ * single-threaded tests. */
+typedef struct {
+	uint64_t shift_clamped;     /* quantize: shift above 15 clamped to 15 */
+	uint64_t negative_shift;    /* quantize: divide branch, shift set to 0 */
+	uint64_t shift_too_small;   /* quantize: shift below -16, candidate dropped (return 1) */
+	uint64_t cmax_zero;         /* quantize: every coefficient 0, candidate dropped (return 2) */
+	uint64_t coef_clipped;      /* quantize: a coefficient clipped to qmin / qmax */
+	uint64_t round_half;        /* quantize: lround of an accumulated error of exactly +-.5 */
+	uint64_t precision_capped;  /* subframe bps <= 17: the precision lowered to 32 - bps - ilog2(order) */
+	uint64_t order_skipped;     /* "don't even try": expected bits >= subframe bps */
+	uint64_t levinson_early;    /* Levinson's error reached 0.0 before max_order */
+	uint64_t wide;              /* evaluated: prediction before shift > 32 bits, or limit */
+	uint64_t limit;             /* evaluated: max residual bps > 32 */
+	uint64_t limit_rejected;    /* evaluated with limit: a residual left (INT32_MIN, INT32_MAX], candidate dropped */
+	uint64_t narrow_wrapped;    /* a partition sum the 32-bit accumulator wrapped */
+} fo_lpc_counters;
+void fo_lpc_counters_get(fo_lpc_counters *out, int reset);
 
 /* ---- decode ---- */
 typedef struct {

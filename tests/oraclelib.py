@@ -31,7 +31,8 @@ class Config(C.Structure):
 class SubframePlan(C.Structure):
     _fields_ = [
         ("type", C.c_int32), ("order", C.c_int32), ("wasted_bits", C.c_int32), ("subframe_bps", C.c_int32),
-        ("qlp_precision", C.c_int32), ("qlp_shift", C.c_int32), ("qlp_coeff", C.c_int32 * FO_MAX_LPC_ORDER),
+        ("qlp_precision", C.c_int32), ("qlp_shift", C.c_int32), ("qlp_negative_shift", C.c_int32),
+        ("qlp_coeff", C.c_int32 * FO_MAX_LPC_ORDER),
         ("rice_method", C.c_int32), ("partition_order", C.c_int32), ("rice_params", C.c_int32 * FO_MAX_PARTITIONS),
         ("estimate_bits", C.c_uint32),
     ]
@@ -40,6 +41,20 @@ class SubframePlan(C.Structure):
 class FramePlan(C.Structure):
     _fields_ = [("channel_assignment", C.c_int32), ("sub", SubframePlan * 8), ("cand", SubframePlan * 4),
                 ("cand_valid", C.c_uint32 * 4)]
+
+
+class LpcCand(C.Structure):
+    _fields_ = [("status", C.c_int32), ("order", C.c_int32), ("precision_tried", C.c_int32), ("precision", C.c_int32),
+                ("shift", C.c_int32), ("negative_shift", C.c_int32), ("qlp", C.c_int32 * FO_MAX_LPC_ORDER)]
+
+
+FO_MAX_LPC_CANDIDATES = FO_MAX_LPC_ORDER * 11
+LPC_COUNTERS = ("shift_clamped", "negative_shift", "shift_too_small", "cmax_zero", "coef_clipped", "round_half", "precision_capped",
+                "order_skipped", "levinson_early", "wide", "limit", "limit_rejected", "narrow_wrapped")
+
+
+class LpcCounters(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in LPC_COUNTERS]
 
 
 class StreamInfo(C.Structure):
@@ -83,6 +98,17 @@ def lib():
         L.fo_window.restype = C.c_int
         L.fo_window.argtypes = [C.POINTER(Apod), C.c_void_p, C.c_int32]
         L.fo_autocorrelation.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
+        L.fo_lpc_candidates.restype = C.c_size_t
+        L.fo_lpc_candidates.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(Config), C.POINTER(LpcCand)]
+        L.fo_lpc_estimate.restype = C.c_uint32
+        L.fo_lpc_estimate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(LpcCand), C.c_uint32, C.c_uint32]
+        L.fo_lpc_counters_get.argtypes = [C.POINTER(LpcCounters), C.c_int]
+        L.fo_max_prediction_value_before_shift.restype = C.c_uint64
+        L.fo_max_prediction_value_before_shift.argtypes = [C.c_uint32, C.c_void_p, C.c_uint32]
+        L.fo_max_residual_bps.restype = C.c_uint32
+        L.fo_max_residual_bps.argtypes = [C.c_uint32, C.c_void_p, C.c_uint32, C.c_int]
+        L.fo_silog2.restype = C.c_uint32
+        L.fo_silog2.argtypes = [C.c_int64]
         _lib = L
     return _lib
 
@@ -103,6 +129,30 @@ def window(apod, length):
     if not lib().fo_window(C.byref(apod), out.ctypes.data, length):
         raise ValueError("unknown apodization type")
     return out
+
+
+def lpc_candidates(autoc, max_order, subframe_bps, blocksize, cfg):
+    """fo_lpc_candidates: the candidates of one autocorrelation row (autoc[0 .. max_order]) in evaluation order."""
+    a = np.ascontiguousarray(autoc, dtype=np.float64)
+    assert a.size >= max_order + 1
+    out = (LpcCand * FO_MAX_LPC_CANDIDATES)()
+    n = lib().fo_lpc_candidates(a.ctypes.data, max_order, subframe_bps, blocksize, C.byref(cfg), out)
+    return list(out[:n])
+
+
+def lpc_counters(reset=False):
+    c = LpcCounters()
+    lib().fo_lpc_counters_get(C.byref(c), int(reset))
+    return {n: getattr(c, n) for n in LPC_COUNTERS}
+
+
+def lpc_flags(subframe_bps, qlp, order, shift):
+    """(wide, limit) as the reference decides them (stream_encoder.c:4601-4617): limit = max residual bps > 32, wide = the
+    prediction before the shift needs more than 32 bits, or limit."""
+    q = np.ascontiguousarray(np.asarray(qlp[:order], dtype=np.int32))
+    limit = lib().fo_max_residual_bps(subframe_bps, q.ctypes.data, order, shift) > 32
+    pred = lib().fo_max_prediction_value_before_shift(subframe_bps, q.ctypes.data, order)
+    return int(limit or lib().fo_silog2(pred) > 32), int(limit)
 
 
 class Encoder:
