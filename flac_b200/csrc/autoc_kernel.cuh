@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(32) k_autoc4(EncK P, const int32_t *__restrict
 	const int item0 = (blockIdx.x - sec * groups) << 5;
 	const int item = min(item0 + lane, nitems - 1);
 	// meta == nullptr: the wasted-bits shift is left to k_lpc (the windowed products and their sums scale EXACTLY by powers of
-	// two, so autoc(x >> w) == autoc(x) * 2^-2w bit for bit) and every signal is analysed -- k_meta then runs concurrently
+	// two, so autoc(x >> w) == autoc(x) * 2^-2w bit for bit) and every signal is analysed -- sigor then stands in for k_meta
 	SigMeta M;
 	M.wasted = 0; M.bps = 1;
 	if(meta) M = meta[item];

@@ -2,7 +2,7 @@
 //
 // Pipeline for a launch of N equal-sized blocks (frames are independent: SURVEY.md §0.1):
 //   k_prep    : de-interleave, mid/side, wasted bits            (stream_encoder.c:3777-3867)
-//   k_autoc   : windowed autocorrelation, one FP64 chain/thread  (lpc.c:68-174)
+//   k_autoc3 / k_autoc4 (autoc_kernel.cuh): windowed FP64 autocorrelation (lpc.c:68-174)
 //   k_lpc     : Levinson-Durbin, order guess, quantisation       (lpc.c:176-314, 1580-1630)
 //   k_search  : fixed scan + candidate residuals + Rice search   (stream_encoder.c:4045-4290, 4701-5075; fixed.c:222-290)
 //   k_emit    : channel assignment, header, residual + Rice bit packing, CRC (stream_encoder.c:3934-4043,
@@ -179,62 +179,6 @@ __global__ void __launch_bounds__(256) k_prep(EncK P, const int32_t *__restrict_
 	}
 }
 
-// ================================================================ k_autoc
-// autoc[l] = sum over ascending i of d[i]*d[i-l], one accumulator per lag (the source order of
-// deduplication/lpc_compute_autocorrelation_intrin.c:5-14 and lpc.c:145-156). The order of
-// additions is fixed, so a chain cannot be split across lanes; instead one THREAD owns one
-// (block, signal, section) chain and keeps all LAGS accumulators plus a LAGS-deep history in
-// registers: LAGS independent DFMAs per sample hide the FP64 latency. float*float products
-// are exact in double, so fma() == mul+add here.
-__device__ __forceinline__ float section_sample(const EncK &P, const DevSection &S, const int32_t *__restrict__ x,
-                                                const float *__restrict__ w, int i)
-{
-	// lpc.c:68-94 FLAC__lpc_window_data / _partial: out = (float)in * window (one float rounding each)
-	if(!S.partial)
-		return __fmul_rn((float)__ldg(x + i), __ldg(w + i));
-	if(i < S.part_size)
-		return __fmul_rn((float)__ldg(x + S.data_shift + i), __ldg(w + i));
-	if(i < 2 * S.part_size)
-		return __fmul_rn((float)__ldg(x + S.data_shift + i), __ldg(w + (P.bs - 2 * S.part_size + i)));
-	return 0.0f;
-}
-
-template <int LAGS>
-__global__ void __launch_bounds__(128) k_autoc(EncK P, const int32_t *__restrict__ sig, const SigMeta *__restrict__ meta,
-                                              const float *__restrict__ windows, const DevSection *__restrict__ secs,
-                                              double *__restrict__ autoc, int nitems)
-{
-	const int gid = blockIdx.x * blockDim.x + threadIdx.x;
-	if(gid >= nitems * P.nsec) return;
-	const int sec = gid / nitems, item = gid - sec * nitems;
-	if(meta[item].bps == 0) return;
-	const DevSection S = secs[sec];
-	const int32_t *x = sig + (size_t)item * P.bs_stride;
-	const float *w = windows + S.win_off;
-	const int n = S.data_len;
-
-	double acc[LAGS], h[LAGS];
-#pragma unroll
-	for(int l = 0; l < LAGS; l++) { acc[l] = 0.0; h[l] = 0.0; }
-
-	for(int base = 0; base < n; base += LAGS) {
-#pragma unroll
-		for(int u = 0; u < LAGS; u++) {
-			const int i = base + u;
-			const float d = (i < n) ? section_sample(P, S, x, w, i) : 0.0f;
-			const double dv = (double)d;
-			const int su = (LAGS - u) % LAGS;  // slot of the newest sample; slot (su+l)%LAGS holds d[i-l]
-			h[su] = dv;
-#pragma unroll
-			for(int l = 0; l < LAGS; l++)
-				acc[l] = fma(dv, h[(su + l) % LAGS], acc[l]);
-		}
-	}
-	double *out = autoc + ((size_t)sec * nitems + item) * P.lag_stride;
-#pragma unroll
-	for(int l = 0; l < LAGS; l++) out[l] = acc[l];
-}
-
 // ================================================================ k_lpc
 
 // lpc.c:1580-1606 FLAC__lpc_compute_expected_bits_per_residual_sample_with_error_scale
@@ -353,8 +297,8 @@ __device__ __forceinline__ int quantize_coefficients(const float (&lp_coeff)[MO]
 }
 
 // One thread per (block, signal, window candidate). Writes nslots/nwin candidate slots.
-// autoc_unshifted: the autocorrelation was taken over the signal BEFORE its wasted bits were shifted out (k_autoc4 running
-// concurrently with k_meta): autoc(x >> w) = autoc(x) * 2^-2w exactly, applied here.
+// autoc_unshifted: the autocorrelation was taken over the signal BEFORE its wasted bits were shifted out (k_autoc4 collecting
+// the wasted-bits OR in place of k_meta): autoc(x >> w) = autoc(x) * 2^-2w exactly, applied here.
 template <int MO>
 __global__ void __launch_bounds__(128) k_lpc(EncK P, const double *__restrict__ autoc, const DevCand *__restrict__ cands,
                                             SigMeta *__restrict__ meta, const uint32_t *__restrict__ sigor, CandDesc *__restrict__ out, int nitems,

@@ -34,7 +34,6 @@ struct Geometry {
 	EncK k{};
 	float *d_windows = nullptr;
 	float *d_secwin = nullptr;  // per-section weight tables over absolute sample indices (k_autoc4), stride bs + kSecwinSlack
-	bool raw_pipeline = false;  // k_meta -> k_autoc4 -> k_lpc -> k_search5 -> k_emit3: every kernel reads the caller's PCM
 	DevSection *d_secs = nullptr;
 	DevCand *d_cands = nullptr;
 	size_t search_smem = 0, emit_smem = 0;  // general kernels
@@ -43,7 +42,6 @@ struct Geometry {
 	size_t search5_smem = 0;
 	int maxord_t = 8;
 	int emit3_rt = 0;           // 0, or R_T of the resident emit kernel (k_emit3)
-	int or_sec = -1;            // a full-length analysis section (k_autoc4 collects the wasted-bits OR there), or -1
 	bool emit3_pair = false;    // more than two channels: k_emit3<PAIR> per channel pair + k_join per frame
 	int pair_words = 0;         // words of a pair's staging region
 	size_t pair_smem = 0, join_smem = 0;
@@ -96,7 +94,7 @@ struct fb200_encoder {
 	// stage-A outputs are double-buffered so that stage A (prep/autoc/lpc) of sub-batch i+1 can run on
 	// s_a concurrently with stage B (search/emit/scan/gather) of sub-batch i on the caller's stream
 	struct WS { int32_t *d_sig; SigMeta *d_meta; int *d_blkflags; double *d_autoc; CandDesc *d_cdesc; uint32_t *d_sigor; } ws[2] = {};
-	cudaStream_t s_a = nullptr, s_meta = nullptr;
+	cudaStream_t s_a = nullptr;
 	// slice mode (the call's blocks fit the workspace): every chunk owns its slice of workspace set 0, so the stage A's of
 	// different chunks are independent and rotate over these streams (s_as[0] == s_a) -- the latency-bound autocorrelation of
 	// a small chunk no longer serialises the pipeline
@@ -104,7 +102,6 @@ struct fb200_encoder {
 	cudaStream_t s_as[kStageAStreams] = {};
 	bool slice_mode = false;
 	std::vector<cudaEvent_t> ev_ca;  // per chunk: stage A done
-	cudaEvent_t ev_meta_fork = nullptr, ev_meta_done = nullptr;
 	cudaEvent_t ev_fork = nullptr, ev_a[2] = {nullptr, nullptr}, ev_b[2] = {nullptr, nullptr};
 	bool ev_b_valid[2] = {false, false};
 	// staging for the host entry point
@@ -153,9 +150,8 @@ struct fb200_encoder {
 	int host_chunks = 12;   // chunks per fb200_encode_host call (FB200_HOST_CHUNKS): copy/compute overlap granularity; on an H100 SXM at 400 W
 	                        // (tools/sweep_host_chunks.py, packed 16-bit, 10 000 blocks) 8-16 are equal within noise and 4 / 24 are ~7 % slower at -8
 	int pipe_chunks = 1;    // sub-batches per fb200_encode_device call (FB200_PIPE_CHUNKS); see fb200_encode_device
-	int debug_path = 0;   // FB200_DEBUG_PATH bit mask (bisecting aid): 1 = k_prep + k_autoc3 instead of k_autoc4, 2 = general search, 4 = general emit, 8 = k_meta instead of the OR fused into k_autoc4,
+	int debug_path = 0;   // FB200_DEBUG_PATH bit mask (bisecting aid): 1 = k_prep + k_autoc3 instead of k_autoc4, 2 = general search, 4 = general emit,
 	                      // 16 = the tiled kernels wherever the general search / emit would run
-	bool use_v1 = false;  // FB200_FORCE_GENERAL_KERNELS=1: run the general kernels for every blocksize (tests)
 	// optional per-kernel CUDA-event timing (bench.py's roofline numbers)
 	bool prof_on = false;
 	std::vector<cudaEvent_t> prof_events;   // consecutive events; kernel id of the interval ending at event i in prof_ids[i]
@@ -273,7 +269,6 @@ static int build_geometry(fb200_encoder *e, int bs, Geometry **out)
 		}
 	}
 	k.nsec = (int)secs.size();
-	g.or_sec = secs.empty() ? -1 : 0;  // every apodization opens with its full-length section
 	k.nwin = (int)cands.size();
 	k.nslots = k.nwin * (k.exhaustive ? (k.max_order > 0 ? k.max_order : 1) : 1) * (k.prec_search ? kQlpPrecisionSteps : 1);
 	if((size_t)k.nsec > e->max_nsec || (size_t)k.nslots > e->max_nslots) {
@@ -338,7 +333,6 @@ static int build_geometry(fb200_encoder *e, int bs, Geometry **out)
 				g.emit3_rt = g.fast_search3; g.emit3_pair = true; g.pair_words = pw; g.pair_smem = need; g.join_smem = needj;
 			}
 		}
-		g.raw_pipeline = g.emit3_rt != 0;
 	}
 	// Where the general kernels would run but their signal / frame does not fit one CTA's shared memory, the tiled kernels
 	// run instead. Strides come from the configured blocksize, so a short last block goes the way its full blocks go.
@@ -368,37 +362,47 @@ static void use_ws(fb200_encoder *e, int b, size_t off_blocks = 0)
 	e->d_cdesc = e->ws[b].d_cdesc + oi * (e->max_nslots ? e->max_nslots : 1);
 }
 
-// Stage A of nb blocks of size g.bs starting at d_pcm: k_prep, k_autoc, k_lpc (writes the current workspace set).
-static int run_stage_a(fb200_encoder *e, Geometry &g, const int32_t *d_pcm, int nb, cudaStream_t st)
+// What a chunk runs, decided once per chunk. k_autoc4, k_search5 and k_emit3 copy raw blocks of the caller's PCM with TMA, so
+// a chunk that starts off 16 bytes (the short last block behind an odd blocksize x channels) takes the planar kernels.
+enum class StageA {
+	fused,   // k_autoc4 on the caller's PCM collects the wasted-bits OR on the way; k_lpc derives wasted bits from it
+	meta,    // k_meta first (no LPC analysis, or loose mid-side: k_autoc4 reads the meta to skip the inactive pair), then k_autoc4
+	planar,  // k_prep's planar copy, then k_autoc3
+};
+enum class Kernel { fast, tiled, general };  // search: k_search5 / tiled / general; emit: k_emit3 / tiled / general + k_scan + k_gather
+struct Route { StageA a; Kernel search, emit; };
+
+static Route route_chunk(const fb200_encoder *e, const Geometry &g, const int32_t *pcm)
+{
+	const int dbg = e->debug_path;
+	const bool aligned = ((uintptr_t)pcm & 15) == 0;
+	Route r;
+	r.search = g.fast_search3 && aligned && !(dbg & 2) ? Kernel::fast : g.tiled_search || (dbg & 16) ? Kernel::tiled : Kernel::general;
+	r.emit = g.emit3_rt && aligned && !(dbg & 4) ? Kernel::fast : g.tiled_emit || (dbg & 16) ? Kernel::tiled : Kernel::general;
+	// stage A may skip the planar copy only when the search and the emit both read the caller's PCM
+	if(r.search != Kernel::fast || r.emit != Kernel::fast || (dbg & 1)) r.a = StageA::planar;
+	else r.a = g.k.nwin > 0 && !g.k.loose_ms ? StageA::fused : StageA::meta;
+	return r;
+}
+
+// Stage A of nb blocks of size g.bs starting at d_pcm: k_prep / k_meta, k_autoc4 / k_autoc3, k_lpc (writes the current
+// workspace set).
+static int run_stage_a(fb200_encoder *e, Geometry &g, StageA how, const int32_t *d_pcm, int nb, cudaStream_t st)
 {
 	EncK k = g.k;
 	const int nitems = nb * k.nsig;
+	const bool fused = how == StageA::fused;
 	prof_mark(e, -1, st);
-	const bool raw = g.raw_pipeline && !e->use_v1 && (e->debug_path & 7) == 0 && ((uintptr_t)d_pcm & 15) == 0;
-	// Wasted-bits detection needs nothing but the OR of a signal's samples. With a full-length analysis section k_autoc4 collects
-	// it on the way (its chains read every sample anyway) and k_lpc derives wasted bits / subframe bps: no kernel reads the block
-	// just for that. Otherwise k_meta does it -- concurrently with k_autoc4 on a second stream when the autocorrelation does not
-	// need the meta data (it does under loose mid-side, to skip the inactive pair); k_lpc joins them.
-	const bool fused = raw && k.nwin > 0 && !k.loose_ms && g.or_sec >= 0 && g.fast_search3 && g.emit3_rt && !(e->debug_path & 8);
-	const bool overlap = !fused && raw && k.nwin > 0 && !k.loose_ms && !e->prof_on;
-	if(fused) {}
-	else if(overlap) {
-		FB_CUDA(cudaEventRecord(e->ev_meta_fork, st));
-		FB_CUDA(cudaStreamWaitEvent(e->s_meta, e->ev_meta_fork, 0));
-		launch_meta(k, d_pcm, e->d_meta, e->d_blkflags, nb, e->s_meta);
-		FB_CUDA(cudaEventRecord(e->ev_meta_done, e->s_meta));
-	}
-	else if(raw) launch_meta(k, d_pcm, e->d_meta, e->d_blkflags, nb, st);  // no planar copy: the fast kernels read the caller's PCM
-	else launch_prep(k, d_pcm, e->d_sig, e->d_meta, e->d_blkflags, nb, st);
+	if(how == StageA::meta) launch_meta(k, d_pcm, e->d_meta, e->d_blkflags, nb, st);
+	else if(how == StageA::planar) launch_prep(k, d_pcm, e->d_sig, e->d_meta, e->d_blkflags, nb, st);
 	prof_mark(e, FB200_PROF_PREP, st);
 	if(!fused) e->launches++;
 	if(k.nwin > 0) {
-		if(raw) launch_autoc4(k, d_pcm, (overlap || fused) ? nullptr : e->d_meta, g.d_secwin, bs_plus_slack(k.bs), g.d_secs, e->d_autoc, nitems, fused ? e->d_sigor : nullptr, g.or_sec, st);
-		else if(e->use_v1) launch_autoc_general(k, e->d_sig, e->d_meta, g.d_windows, g.d_secs, e->d_autoc, nitems, st);
-		else launch_autoc3(k, e->d_sig, e->d_meta, g.d_windows, g.d_secs, e->d_autoc, nitems, st);
+		// k_autoc4 ORs section 0's samples: every apodization opens with its full-length section
+		if(how == StageA::planar) launch_autoc3(k, e->d_sig, e->d_meta, g.d_windows, g.d_secs, e->d_autoc, nitems, st);
+		else launch_autoc4(k, d_pcm, fused ? nullptr : e->d_meta, g.d_secwin, bs_plus_slack(k.bs), g.d_secs, e->d_autoc, nitems, fused ? e->d_sigor : nullptr, 0, st);
 		prof_mark(e, FB200_PROF_AUTOC, st);
-		if(overlap) FB_CUDA(cudaStreamWaitEvent(st, e->ev_meta_done, 0));
-		launch_lpc(k, e->d_autoc, g.d_cands, e->d_meta, fused ? e->d_sigor : nullptr, e->d_cdesc, nitems, (overlap || fused) ? 1 : 0, st);
+		launch_lpc(k, e->d_autoc, g.d_cands, e->d_meta, fused ? e->d_sigor : nullptr, e->d_cdesc, nitems, fused ? 1 : 0, st);
 		prof_mark(e, FB200_PROF_LPC, st);
 		e->launches += 2;
 	}
@@ -406,9 +410,23 @@ static int run_stage_a(fb200_encoder *e, Geometry &g, const int32_t *d_pcm, int 
 	return FB200_OK;
 }
 
-// Stage B: search + emit (reads the current workspace set). Regular blocksizes: k_search4 + k_emit3 (frames go straight
-// to their final offsets); everything else: the general k_search + k_emit + k_scan + k_gather.
-static int run_stage_b(fb200_encoder *e, Geometry &g, const int32_t *d_pcm, int nb, uint32_t first_frame, uint64_t frame_index0,
+// Grows a pair of stage-B staging arrays to `regions` regions of `words` words and one bit count per region. Growing
+// synchronises `st` first (once per geometry): kernels queued on it may still use the old arrays.
+static int grow_staging(cudaStream_t st, uint32_t **d_words, uint32_t **d_bits, size_t *cap_words, size_t regions, size_t words)
+{
+	const size_t need = regions * words;
+	if(need <= *cap_words) return FB200_OK;
+	FB_CUDA(cudaStreamSynchronize(st));
+	cudaFree(*d_words); cudaFree(*d_bits); *d_words = nullptr; *d_bits = nullptr; *cap_words = 0;
+	FB_CUDA(cudaMalloc(d_words, need * sizeof(uint32_t)));
+	FB_CUDA(cudaMalloc(d_bits, regions * sizeof(uint32_t)));
+	*cap_words = need;
+	return FB200_OK;
+}
+
+// Stage B: search + emit (reads the current workspace set). k_emit3 writes frames straight to their final offsets; the tiled
+// and general emits write slots that k_scan + k_gather place.
+static int run_stage_b(fb200_encoder *e, Geometry &g, const Route &r, const int32_t *d_pcm, int nb, uint32_t first_frame, uint64_t frame_index0,
                        uint8_t *d_out, size_t out_cap, unsigned long long *d_offsets, cudaStream_t st)
 {
 	EncK k = g.k;
@@ -417,14 +435,11 @@ static int run_stage_b(fb200_encoder *e, Geometry &g, const int32_t *d_pcm, int 
 	k.file_blocks = (int)e->file_blocks;
 	k.frame_no = e->files_frame_no;
 	const int nitems = nb * k.nsig;
+	int rc;
 	prof_mark(e, -1, st);
-	// k_search5 copies raw blocks with TMA: a chunk that starts off 16 bytes (the short last block behind an odd blocksize x
-	// channels) takes the planar path, as stage A and the emit do
-	const bool fast_search = g.fast_search3 && !e->use_v1 && !(e->debug_path & 2) && ((uintptr_t)d_pcm & 15) == 0;
-	const bool tiled_search = !fast_search && (g.tiled_search || (e->debug_path & 16));
 	auto search = [&](const EncK &kk) {
-		if(fast_search) launch_search5(kk, g.fast_search3, g.maxord_t, g.search_wps, g.search5_smem, d_pcm, e->d_meta, e->d_cdesc, e->d_plans, nb, st);
-		else if(tiled_search) launch_search_tiled(kk, e->d_sig, e->d_meta, e->d_cdesc, e->d_plans, nitems, st);
+		if(r.search == Kernel::fast) launch_search5(kk, g.fast_search3, g.maxord_t, g.search_wps, g.search5_smem, d_pcm, e->d_meta, e->d_cdesc, e->d_plans, nb, st);
+		else if(r.search == Kernel::tiled) launch_search_tiled(kk, e->d_sig, e->d_meta, e->d_cdesc, e->d_plans, nitems, st);
 		else launch_search_general(kk, g.search_smem, e->d_sig, e->d_meta, e->d_cdesc, e->d_plans, nitems, st);
 	};
 	search(k);
@@ -439,7 +454,7 @@ static int run_stage_b(fb200_encoder *e, Geometry &g, const int32_t *d_pcm, int 
 		e->launches += 2;
 	}
 	prof_mark(e, FB200_PROF_SEARCH, st);
-	if(g.emit3_rt && !e->use_v1 && !(e->debug_path & 4) && ((uintptr_t)d_pcm & 15) == 0) {
+	if(r.emit == Kernel::fast) {
 		if((++e->epoch & kLbEpochMask) == 0) {
 			FB_CUDA(cudaMemsetAsync(e->d_lookback, 0, (size_t)e->max_blocks * sizeof(unsigned long long), st));
 			e->epoch = 1;
@@ -452,15 +467,8 @@ static int run_stage_b(fb200_encoder *e, Geometry &g, const int32_t *d_pcm, int 
 		a.nb = nb; a.chan_assign_out = e->d_chan_assign; a.err = e->d_err;
 		a.stage = nullptr; a.stage_bits = nullptr; a.pair_words = g.pair_words; a.join_words = k.emit3_words;
 		if(g.emit3_pair) {
-			const size_t npairs = ((size_t)k.channels + 1) / 2;
-			const size_t need = (size_t)e->max_blocks * npairs * (size_t)g.pair_words;
-			if(need > e->d_stage_words) {  // first use with this geometry (synchronous, once)
-				FB_CUDA(cudaStreamSynchronize(st));
-				cudaFree(e->d_stage); cudaFree(e->d_stage_bits); e->d_stage = nullptr; e->d_stage_bits = nullptr; e->d_stage_words = 0;
-				FB_CUDA(cudaMalloc(&e->d_stage, need * sizeof(uint32_t)));
-				FB_CUDA(cudaMalloc(&e->d_stage_bits, (size_t)e->max_blocks * npairs * sizeof(uint32_t)));
-				e->d_stage_words = need;
-			}
+			const size_t regions = (size_t)e->max_blocks * (((size_t)k.channels + 1) / 2);
+			if((rc = grow_staging(st, &e->d_stage, &e->d_stage_bits, &e->d_stage_words, regions, (size_t)g.pair_words)) != FB200_OK) return rc;
 			a.stage = e->d_stage; a.stage_bits = e->d_stage_bits;
 			launch_emit3_pairs(k, g.emit3_rt, g.maxord_t, g.pair_smem, g.join_smem, a, nb, st);
 		}
@@ -471,15 +479,9 @@ static int run_stage_b(fb200_encoder *e, Geometry &g, const int32_t *d_pcm, int 
 		e->launches += 2;
 	}
 	else {
-		if(g.tiled_emit || (e->debug_path & 16)) {
-			const size_t need = (size_t)e->max_blocks * k.channels * (size_t)g.sub_words;
-			if(need > e->d_tstage_words) {  // first use with this geometry (synchronous, once)
-				FB_CUDA(cudaStreamSynchronize(st));
-				cudaFree(e->d_tstage); cudaFree(e->d_tstage_bits); e->d_tstage = nullptr; e->d_tstage_bits = nullptr; e->d_tstage_words = 0;
-				FB_CUDA(cudaMalloc(&e->d_tstage, need * sizeof(uint32_t)));
-				FB_CUDA(cudaMalloc(&e->d_tstage_bits, (size_t)e->max_blocks * k.channels * sizeof(uint32_t)));
-				e->d_tstage_words = need;
-			}
+		if(r.emit == Kernel::tiled) {
+			const size_t regions = (size_t)e->max_blocks * k.channels;
+			if((rc = grow_staging(st, &e->d_tstage, &e->d_tstage_bits, &e->d_tstage_words, regions, (size_t)g.sub_words)) != FB200_OK) return rc;
 			launch_emit_tiled(k, e->d_sig, e->d_blkflags, e->d_plans, e->d_tstage, e->d_tstage_bits, g.sub_words, g.sub_cap_bits, e->d_slots,
 			                  e->d_frame_bytes, e->d_chan_assign, e->d_err, nb, st);
 			e->launches++;
@@ -499,6 +501,19 @@ static int run_stage_b(fb200_encoder *e, Geometry &g, const int32_t *d_pcm, int 
 // pcm: the chunk's first sample, or null for d_pcm_base + first full blocks (a group of short tails lies elsewhere)
 struct PipeChunk { uint64_t first; uint32_t nb; uint32_t blocksize; cudaEvent_t wait_before_a; const int32_t *pcm = nullptr; };
 
+// A call's nfull full blocks in chunks of ceil(nfull / parts) blocks, at least min_chunk and at most max_blocks each. The
+// caller appends its short blocks.
+static std::vector<PipeChunk> full_block_chunks(const fb200_encoder *e, uint64_t nfull, int parts, uint64_t min_chunk)
+{
+	uint64_t chunk = (nfull + parts - 1) / parts;
+	if(chunk < min_chunk) chunk = min_chunk;
+	if(chunk > e->max_blocks) chunk = e->max_blocks;
+	std::vector<PipeChunk> chunks;
+	for(uint64_t done = 0; done < nfull; done += chunk)
+		chunks.push_back(PipeChunk{done, (uint32_t)((nfull - done) < chunk ? (nfull - done) : chunk), e->cfg.blocksize, nullptr});
+	return chunks;
+}
+
 // Enqueue chunk `idx` of a call: stage A on a stage-A stream, stage B on `sb`. Slice mode: the chunk works in its own slice of
 // workspace set 0; otherwise consecutive chunks alternate between the two sets and wait for the set's previous user.
 static cudaStream_t stage_a_stream(fb200_encoder *e, size_t idx) { return e->slice_mode ? e->s_as[idx % fb200_encoder::kStageAStreams] : e->s_a; }
@@ -516,7 +531,8 @@ static int enqueue_chunk(fb200_encoder *e, size_t idx, const PipeChunk &c, const
 	if(!e->slice_mode && e->ev_b_valid[b]) FB_CUDA(cudaStreamWaitEvent(sa, e->ev_b[b], 0));  // stage B two chunks ago is done with this set
 	use_ws(e, b, e->slice_mode ? (size_t)c.first : 0);
 	const int32_t *pcm = c.pcm ? c.pcm : d_pcm_base + (size_t)c.first * bs * ch;
-	if((rc = run_stage_a(e, *g, pcm, (int)c.nb, sa)) != FB200_OK) return rc;
+	const Route r = route_chunk(e, *g, pcm);
+	if((rc = run_stage_a(e, *g, r.a, pcm, (int)c.nb, sa)) != FB200_OK) return rc;
 	cudaEvent_t done_a = e->ev_a[b];
 	if(e->slice_mode) {
 		while(e->ev_ca.size() <= idx) {
@@ -528,7 +544,7 @@ static int enqueue_chunk(fb200_encoder *e, size_t idx, const PipeChunk &c, const
 	}
 	FB_CUDA(cudaEventRecord(done_a, sa));
 	FB_CUDA(cudaStreamWaitEvent(sb, done_a, 0));
-	if((rc = run_stage_b(e, *g, pcm, (int)c.nb, first_frame_number, c.first, d_out, out_cap, d_offsets, sb)) != FB200_OK) return rc;
+	if((rc = run_stage_b(e, *g, r, pcm, (int)c.nb, first_frame_number, c.first, d_out, out_cap, d_offsets, sb)) != FB200_OK) return rc;
 	if(!e->slice_mode) {
 		FB_CUDA(cudaEventRecord(e->ev_b[b], sb));
 		e->ev_b_valid[b] = true;
@@ -536,11 +552,14 @@ static int enqueue_chunk(fb200_encoder *e, size_t idx, const PipeChunk &c, const
 	return FB200_OK;
 }
 
-// after the call's set-up work was enqueued on `st`: every stage-A stream starts behind it
-static int fork_stage_a(fb200_encoder *e, cudaStream_t st)
+// Starts a call's pipeline of nblocks blocks after its set-up work was enqueued on `st`: slice mode when the blocks fit the
+// workspace, every stage-A stream of that mode behind `st`, and no wait on a previous call's stage B.
+static int fork_stage_a(fb200_encoder *e, uint64_t nblocks, cudaStream_t st)
 {
+	e->slice_mode = nblocks <= e->max_blocks;
 	FB_CUDA(cudaEventRecord(e->ev_fork, st));
 	for(int i = 0; i < (e->slice_mode ? fb200_encoder::kStageAStreams : 1); i++) FB_CUDA(cudaStreamWaitEvent(e->s_as[i], e->ev_fork, 0));
+	e->ev_b_valid[0] = e->ev_b_valid[1] = false;
 	return FB200_OK;
 }
 
@@ -789,9 +808,7 @@ static int create_impl(const fb200_encoder_config *cfg_in, int device, uint32_t 
 	bool streams_ok = true;
 	for(int i = 0; i < fb200_encoder::kStageAStreams; i++) streams_ok = streams_ok && cudaStreamCreateWithFlags(&e->s_as[i], cudaStreamNonBlocking) == cudaSuccess;
 	e->s_a = e->s_as[0];
-	if(!streams_ok || cudaStreamCreateWithFlags(&e->s_meta, cudaStreamNonBlocking) != cudaSuccess ||
-	   cudaEventCreateWithFlags(&e->ev_meta_fork, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&e->ev_meta_done, cudaEventDisableTiming) != cudaSuccess ||
-	   cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
+	if(!streams_ok || cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
 	   cudaEventCreateWithFlags(&e->ev_a[0], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&e->ev_a[1], cudaEventDisableTiming) != cudaSuccess ||
 	   cudaEventCreateWithFlags(&e->ev_b[0], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&e->ev_b[1], cudaEventDisableTiming) != cudaSuccess ||
 	   cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) {
@@ -819,8 +836,6 @@ static int create_impl(const fb200_encoder_config *cfg_in, int device, uint32_t 
 		}
 	}
 	{
-		const char *env = getenv("FB200_FORCE_GENERAL_KERNELS");
-		e->use_v1 = env && env[0] == '1';
 		const char *dp = getenv("FB200_DEBUG_PATH");
 		if(dp) e->debug_path = atoi(dp);
 		const char *hc = getenv("FB200_HOST_CHUNKS");
@@ -852,9 +867,6 @@ void fb200_encoder_destroy(fb200_encoder *e)
 	if(e->ev_fork) cudaEventDestroy(e->ev_fork);
 	for(int i = 0; i < fb200_encoder::kStageAStreams; i++) if(e->s_as[i]) cudaStreamDestroy(e->s_as[i]);
 	for(cudaEvent_t ev : e->ev_ca) cudaEventDestroy(ev);
-	if(e->s_meta) cudaStreamDestroy(e->s_meta);
-	if(e->ev_meta_fork) cudaEventDestroy(e->ev_meta_fork);
-	if(e->ev_meta_done) cudaEventDestroy(e->ev_meta_done);
 	cudaFree(e->d_plans); cudaFree(e->d_slots); cudaFree(e->d_frame_bytes); cudaFree(e->d_chan_assign);
 	cudaFree(e->d_running); cudaFree(e->d_err); cudaFree(e->d_redo); cudaFree(e->d_stage); cudaFree(e->d_stage_bits);
 	cudaFree(e->d_tstage); cudaFree(e->d_tstage_bits);
@@ -902,7 +914,7 @@ int fb200_encode_device(fb200_encoder *e, const int32_t *d_pcm, uint64_t samples
 	if(e->verify) return refuse_unverified();
 	FB_CUDA(cudaSetDevice(e->device));
 	cudaStream_t st = (cudaStream_t)cuda_stream;
-	const uint32_t bs = e->cfg.blocksize, ch = e->cfg.channels;
+	const uint32_t bs = e->cfg.blocksize;
 	const uint64_t nfull = samples / bs;
 	const uint32_t tail = (uint32_t)(samples % bs);
 	if(nframes) *nframes = (uint32_t)(nfull + (tail ? 1 : 0));
@@ -915,16 +927,9 @@ int fb200_encode_device(fb200_encoder *e, const int32_t *d_pcm, uint64_t samples
 	// per call is fastest at -5 (1.24 ms per step vs 1.34 with 4 sub-batches) and no sub-batch count wins at -8 (3.83-3.89 ms for
 	// 1-4) -- every kernel is more efficient at full batch size than the overlap wins back, so the default is as few
 	// sub-batches as the workspace allows.
-	uint64_t chunk = (nfull + e->pipe_chunks - 1) / e->pipe_chunks;
-	if(chunk < 512) chunk = 512;
-	if(chunk > e->max_blocks) chunk = e->max_blocks;
-	std::vector<PipeChunk> chunks;
-	for(uint64_t done = 0; done < nfull; done += chunk)
-		chunks.push_back(PipeChunk{done, (uint32_t)((nfull - done) < chunk ? (nfull - done) : chunk), bs, nullptr});
+	std::vector<PipeChunk> chunks = full_block_chunks(e, nfull, e->pipe_chunks, 512);
 	if(tail) chunks.push_back(PipeChunk{nfull, 1, tail, nullptr});  // short last block: own windows / header blocksize (stream_encoder.c:1703-1711)
-	e->slice_mode = nfull + (tail ? 1 : 0) <= e->max_blocks;
-	{ const int rc = fork_stage_a(e, st); if(rc != FB200_OK) return rc; }
-	e->ev_b_valid[0] = e->ev_b_valid[1] = false;
+	{ const int rc = fork_stage_a(e, nfull + (tail ? 1 : 0), st); if(rc != FB200_OK) return rc; }
 	for(size_t i = 0; i < chunks.size(); i++) {
 		const int rc = enqueue_chunk(e, i, chunks[i], d_pcm, first_frame_number, d_out, out_capacity, offs, st);
 		if(rc != FB200_OK) return rc;
@@ -989,12 +994,7 @@ static int encode_host_impl(fb200_encoder *e, const void *pcm_any, uint32_t byte
 	if(!e->s_h2d) FB_CUDA(cudaStreamCreateWithFlags(&e->s_h2d, cudaStreamNonBlocking));
 	if(!e->s_d2h) FB_CUDA(cudaStreamCreateWithFlags(&e->s_d2h, cudaStreamNonBlocking));
 	// chunking: host_chunks (default 12) chunks per call, between 256 blocks and the launch capacity; the short last block is its own chunk
-	uint64_t chunk = (nfull + e->host_chunks - 1) / e->host_chunks;
-	if(chunk < 256) chunk = 256;
-	if(chunk > e->max_blocks) chunk = e->max_blocks;
-	std::vector<PipeChunk> chunks;
-	for(uint64_t done = 0; done < nfull; done += chunk)
-		chunks.push_back(PipeChunk{done, (uint32_t)((nfull - done) < chunk ? (nfull - done) : chunk), bs, nullptr});
+	std::vector<PipeChunk> chunks = full_block_chunks(e, nfull, e->host_chunks, 256);
 	if(tail) chunks.push_back(PipeChunk{nfull, 1, tail, nullptr});
 	const size_t used = chunks.size();
 	if(used > e->h_totals_cap) {
@@ -1012,9 +1012,7 @@ static int encode_host_impl(fb200_encoder *e, const void *pcm_any, uint32_t byte
 	cudaStream_t sc = e->stream;
 	FB_CUDA(cudaMemsetAsync(e->d_running, 0, 2 * sizeof(unsigned long long), sc));
 	FB_CUDA(cudaMemsetAsync(e->d_err, 0, sizeof(int), sc));
-	e->slice_mode = nfr <= e->max_blocks;
-	{ const int rc = fork_stage_a(e, sc); if(rc != FB200_OK) return rc; }  // the error word is cleared before any kernel of this call may set it
-	e->ev_b_valid[0] = e->ev_b_valid[1] = false;
+	{ const int rc = fork_stage_a(e, nfr, sc); if(rc != FB200_OK) return rc; }  // the error word is cleared before any kernel of this call may set it
 	for(size_t ci = 0; ci < used; ci++) {
 		PipeChunk &c = chunks[ci];
 		const size_t off_elems = (size_t)c.first * bs * ch;
@@ -1158,14 +1156,7 @@ static int encode_files_impl(fb200_encoder *e, const void *pcm, uint32_t bytes_p
 			fb += nfull;
 		}
 	}
-	std::vector<PipeChunk> chunks;
-	{
-		uint64_t chunk = (nfull_all + e->pipe_chunks - 1) / e->pipe_chunks;
-		if(chunk < 512) chunk = 512;
-		if(chunk > e->max_blocks) chunk = e->max_blocks;
-		for(uint64_t done = 0; done < nfull_all; done += chunk)
-			chunks.push_back(PipeChunk{done, (uint32_t)((nfull_all - done) < chunk ? (nfull_all - done) : chunk), (uint32_t)bs, nullptr});
-	}
+	std::vector<PipeChunk> chunks = full_block_chunks(e, nfull_all, e->pipe_chunks, 512);
 	const size_t nfull_chunks = chunks.size();
 	std::vector<uint64_t> tail_pcm;  // element offset of each tail chunk in the compacted layout
 	uint64_t compact = nfull_all * bs * ch;
@@ -1376,10 +1367,7 @@ static int encode_files_impl(fb200_encoder *e, const void *pcm, uint32_t bytes_p
 		                  reinterpret_cast<uint32_t *>(d + o_rgpk), e->s_rg);
 		e->launches++;
 	}
-	// slice mode decides which stage-A streams fork_stage_a holds behind the input: it must be set first
-	e->slice_mode = nv <= e->max_blocks;
-	if((rc = fork_stage_a(e, st)) != FB200_OK) return rc;
-	e->ev_b_valid[0] = e->ev_b_valid[1] = false;
+	if((rc = fork_stage_a(e, nv, st)) != FB200_OK) return rc;
 	e->files_frame_no = reinterpret_cast<const uint32_t *>(d + o_fno);
 	for(size_t i = 0; i < chunks.size(); i++)
 		if((rc = enqueue_chunk(e, i, chunks[i], e->d_pcm, 0, e->d_out, vcap, d_voff, st)) != FB200_OK) return rc;

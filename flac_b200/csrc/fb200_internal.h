@@ -175,7 +175,6 @@ __host__ __device__ inline size_t emit3_smem_bytes(int bs, int R_T, int nch, int
 void launch_unpack(const void *packed, int bytes_per_sample, int32_t *pcm, unsigned long long n, int bps, int *err, cudaStream_t st);
 void launch_meta(const EncK &k, const int32_t *pcm, SigMeta *meta, int *blkflags, int nb, cudaStream_t st);
 void launch_prep(const EncK &k, const int32_t *pcm, int32_t *sig, SigMeta *meta, int *blkflags, int nb, cudaStream_t st);
-void launch_autoc_general(const EncK &k, const int32_t *sig, const SigMeta *meta, const float *windows, const DevSection *secs, double *autoc, int nitems, cudaStream_t st);
 void launch_minbr_flags(const EncK &k, const SubframePlan *plans, const int *blkflags, int nb, int *flags, cudaStream_t st);
 void launch_debug_evaluate(const EncK &k, const int32_t *sig, const SigMeta *meta, const CandDesc *cands, uint32_t *absr, uint32_t *est, int n);
 void launch_lpc(const EncK &k, const double *autoc, const DevCand *cands, SigMeta *meta, const uint32_t *sigor, CandDesc *cdesc, int nitems, int autoc_unshifted, cudaStream_t st);

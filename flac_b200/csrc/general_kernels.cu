@@ -22,22 +22,6 @@ void launch_unpack(const void *packed, int bytes_per_sample, int32_t *pcm, unsig
 	else k_unpack<3><<<grid, 256, 0, st>>>(static_cast<const uint8_t *>(packed), pcm, n, bps, err);
 }
 
-template <int LAGS>
-static void autoc_general(const EncK &k, const int32_t *sig, const SigMeta *meta, const float *windows, const DevSection *secs, double *autoc, int nitems, cudaStream_t st)
-{
-	const int total = nitems * k.nsec;
-	k_autoc<LAGS><<<(total + 127) / 128, 128, 0, st>>>(k, sig, meta, windows, secs, autoc, nitems);
-}
-
-void launch_autoc_general(const EncK &k, const int32_t *sig, const SigMeta *meta, const float *windows, const DevSection *secs, double *autoc, int nitems, cudaStream_t st)
-{
-	if(k.lags <= 7) autoc_general<7>(k, sig, meta, windows, secs, autoc, nitems, st);
-	else if(k.lags <= 9) autoc_general<9>(k, sig, meta, windows, secs, autoc, nitems, st);
-	else if(k.lags <= 13) autoc_general<13>(k, sig, meta, windows, secs, autoc, nitems, st);
-	else if(k.lags <= 17) autoc_general<17>(k, sig, meta, windows, secs, autoc, nitems, st);
-	else autoc_general<33>(k, sig, meta, windows, secs, autoc, nitems, st);
-}
-
 void launch_minbr_flags(const EncK &k, const SubframePlan *plans, const int *blkflags, int nb, int *flags, cudaStream_t st)
 {
 	k_minbr_flags<<<(nb + 127) / 128, 128, 0, st>>>(k, plans, blkflags, nb, flags);

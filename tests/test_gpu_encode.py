@@ -162,9 +162,9 @@ def test_big_batch_property_round_trip():
 
 @pytest.mark.parametrize("level,ch,bps", [(8, 2, 16), (5, 2, 24), (5, 1, 16), (2, 2, 16), (8, 2, 24)])
 def test_general_kernels_equal_fast_kernels(monkeypatch, level, ch, bps):
-    """FB200_FORCE_GENERAL_KERNELS=1 runs the general kernels (any blocksize) on a blocksize the fast kernels
-    (k_autoc3 / k_search4 / k_emit3) normally take: both must give the oracle's frames."""
-    monkeypatch.setenv("FB200_FORCE_GENERAL_KERNELS", "1")
+    """FB200_DEBUG_PATH=7 runs the general kernels (k_prep + k_autoc3, k_search, k_emit + k_scan + k_gather: any blocksize) on a
+    blocksize the fast kernels (k_autoc4 / k_search5 / k_emit3) normally take: both must give the oracle's frames."""
+    monkeypatch.setenv("FB200_DEBUG_PATH", "7")
     x = signals.music_like(4096 * 3 + 55, ch, bps, 44100, seed=17)
     got = _gpu_frames(x, bps, 44100, level)
     _assert_same(got, _oracle_frames(x, bps, 44100, level), "general kernels")

@@ -126,9 +126,9 @@ def test_general_kernels(bs):
         check(x, bps, 44100, level, bs, "general", what=kind)
 
 
-@pytest.mark.parametrize("env,value", [("FB200_FORCE_GENERAL_KERNELS", "1"), ("FB200_DEBUG_PATH", "22")], ids=["general", "tiled"])
+@pytest.mark.parametrize("env,value", [("FB200_DEBUG_PATH", "7"), ("FB200_DEBUG_PATH", "22")], ids=["debug_path_7", "tiled"])
 def test_forced_paths_on_regular_blocksizes(monkeypatch, env, value):
-    """The general kernels (FB200_FORCE_GENERAL_KERNELS=1) and the tiled kernels (FB200_DEBUG_PATH=22) on blocksizes the fast
+    """The general kernels (FB200_DEBUG_PATH=7) and the tiled kernels (FB200_DEBUG_PATH=22) on blocksizes the fast
     kernels would take."""
     monkeypatch.setenv(env, value)
     for k, bps, ch, kind, rng in path_cells(len(value)):
@@ -146,7 +146,7 @@ def constant_blocks(bs, ch, bps, seed):
     return x
 
 
-PATHS = [("fast", 4096, None), ("fast", 1152, None), ("general", 1000, None), ("general", 4096, ("FB200_FORCE_GENERAL_KERNELS", "1")),
+PATHS = [("fast", 4096, None), ("fast", 1152, None), ("general", 1000, None), ("general", 4096, ("FB200_DEBUG_PATH", "7")),
          ("general", 4608, ("FB200_DEBUG_PATH", "22"))]
 
 

@@ -9,7 +9,7 @@ test_oracle_lpc_edges.py pins against the reference at these inputs.
   * Whole encodes of the PCM inputs of lpcedges.py (negative shifts, 64-bit and checked residuals, a checked residual that
     leaves int32, 32-bit partition sums that wrap, a 25-bit side channel) equal the oracle frame for frame on every stage-B
     path: k_search5 + k_emit3 (1-2 channels), k_search5 + k_emit3<PAIR> + k_join (5 and 7 channels), the general kernels
-    (natural blocksizes and FB200_FORCE_GENERAL_KERNELS=1) and the tiled kernels (FB200_DEBUG_PATH=22, and 16384 / 40000).
+    (natural blocksizes and FB200_DEBUG_PATH=7) and the tiled kernels (FB200_DEBUG_PATH=22, and 16384 / 40000).
     The encoder's chosen plans are compared too: on the 5-channel input each of the join, general and tiled paths chooses LPC
     subframes with a 64-bit residual, so the emit's wide residual runs there."""
 import math
@@ -151,7 +151,7 @@ def chosen_wide_lpc(x, bps, level, bs, **cfg):
     return got, want
 
 
-PATHS = [("natural", None), ("general", ("FB200_FORCE_GENERAL_KERNELS", "1")), ("tiled", ("FB200_DEBUG_PATH", "22"))]
+PATHS = [("natural", None), ("debug_path_7", ("FB200_DEBUG_PATH", "7")), ("tiled", ("FB200_DEBUG_PATH", "22"))]
 
 
 @pytest.mark.parametrize("env", PATHS, ids=[p[0] for p in PATHS])
