@@ -210,6 +210,39 @@ def pcm_decode_options(kind="wave", subformat=None, md5=True, channel_map_none=F
                             1 if md5 else 0, 1 if channel_map_none else 0)
 
 
+RGS_LIMIT_NONE, RGS_LIMIT_PEAK, RGS_LIMIT_HARD = range(3)
+RGS_APPLIED, RGS_NO_TAGS, RGS_BPS, RGS_GAIN, RGS_NOT_DECODED = range(5)
+
+
+class ReplayGainSynthesis(C.Structure):
+    """Mirror of fb200_replaygain_synthesis: what flac -d --apply-replaygain-which-is-not-lossless[=SPEC] applies, and whether a
+    list of whole files is one invocation (per_file 0: the dither generator runs on from file to file) or one per file."""
+    _fields_ = [("preamp", C.c_double), ("album", C.c_uint32), ("limiter", C.c_uint32), ("noise_shaping", C.c_uint32), ("per_file", C.c_uint32)]
+
+
+class ReplayGainSynthesisInfo(C.Structure):
+    """Mirror of fb200_replaygain_synthesis_info: the tool's decision for one container and where its dither draws lie."""
+    _fields_ = [("status", C.c_uint32), ("album_used", C.c_uint32), ("reference", C.c_double), ("gain", C.c_double), ("peak", C.c_double),
+                ("scale", C.c_double), ("first_draw", C.c_uint64), ("draws", C.c_uint64)]
+
+
+def replaygain_synthesis(spec=None, per_file=False):
+    """fb200_replaygain_synthesis_parse: the option's SPEC (None: the option without '='). Raises on a spec the tool rejects."""
+    rg = ReplayGainSynthesis()
+    _check(lib().fb200_replaygain_synthesis_parse(None if spec is None else spec.encode(), C.byref(rg)))
+    rg.per_file = 1 if per_file else 0
+    return rg
+
+
+def replaygain_synthesis_file(blob, spec=None):
+    """fb200_replaygain_synthesis_file: the tool's decision and scale for one .flac (its metadata only)."""
+    rg = spec if isinstance(spec, ReplayGainSynthesis) else replaygain_synthesis(spec)
+    b = np.frombuffer(bytes(blob), dtype=np.uint8)
+    info = ReplayGainSynthesisInfo()
+    _check(lib().fb200_replaygain_synthesis_file(b.ctypes.data, b.size, C.byref(rg), C.byref(info)))
+    return info
+
+
 def pcm_header(channels, bits_per_sample, sample_rate, samples, channel_mask=0, **opts):
     """fb200_pcm_header: the header flac -d writes for these facts (channel_mask: the file's tag, 0 for none). Raises where the
     tool refuses the kind for this length (code -2)."""
@@ -290,6 +323,15 @@ def lib():
     L.fb200_replaygain_rewrite_head.argtypes = [C.c_void_p, C.c_uint64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_uint64,
                                                 C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32)]
     L.fb200_pcm_header.restype = C.c_int
+    L.fb200_replaygain_synthesis_parse.restype = C.c_int
+    L.fb200_replaygain_synthesis_parse.argtypes = [C.c_char_p, C.POINTER(ReplayGainSynthesis)]
+    L.fb200_replaygain_synthesis_file.restype = C.c_int
+    L.fb200_replaygain_synthesis_file.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(ReplayGainSynthesis), C.POINTER(ReplayGainSynthesisInfo)]
+    L.fb200_debug_tanh.restype = C.c_int
+    L.fb200_debug_tanh.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_int]
+    L.fb200_debug_replaygain_synthesis.restype = C.c_int
+    L.fb200_debug_replaygain_synthesis.argtypes = [C.c_int, C.c_void_p, C.c_uint32, C.c_uint64, C.c_void_p, C.c_uint32, C.c_uint32, C.c_double,
+                                                   C.c_uint32, C.c_uint32, C.c_uint64, C.c_void_p]
     L.fb200_pcm_header.argtypes = [C.POINTER(PcmDecodeOptions), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_void_p, C.c_uint32,
                                    C.POINTER(C.c_uint32)]
     L.fb200_encoder_get_verify.restype = C.c_int
@@ -349,6 +391,13 @@ def lib():
         L.fb200_decode_pcm_files_device.restype = C.c_int
         L.fb200_decode_pcm_files_device.argtypes = [C.c_void_p, C.POINTER(PcmDecodeOptions), C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64,
                                                     C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p]
+        L.fb200_decode_pcm_files_replaygain_host.restype = C.c_int
+        L.fb200_decode_pcm_files_replaygain_host.argtypes = [C.c_void_p, C.POINTER(PcmDecodeOptions), C.POINTER(ReplayGainSynthesis), C.c_void_p,
+                                                             C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p]
+        L.fb200_decode_pcm_files_replaygain_device.restype = C.c_int
+        L.fb200_decode_pcm_files_replaygain_device.argtypes = [C.c_void_p, C.POINTER(PcmDecodeOptions), C.POINTER(ReplayGainSynthesis), C.c_void_p,
+                                                               C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p,
+                                                               C.c_void_p]
         L.fb200_add_replaygain_flac_files_host.restype = C.c_int
         L.fb200_add_replaygain_flac_files_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(AddReplayGainOptions),
                                                            C.c_void_p, C.c_size_t, C.c_void_p]
@@ -618,6 +667,37 @@ def decode_pcm_files(blobs, kind="wave", device=0, **opts):
         return dec.decode_pcm_files(kind=kind, **opts)
     finally:
         dec.close()
+
+
+def decode_pcm_files_replaygain(blobs, spec=None, per_file=False, kind="wave", device=0, **opts):
+    """flac -d --apply-replaygain-which-is-not-lossless[=SPEC] *.flac in one call: as decode_pcm_files, with ReplayGain applied
+    where the tool applies it. per_file False: the list is one invocation of the tool (its dither generator runs on from file to
+    file, in list order); True: one invocation per file. Returns, in input (or range) order, (container bytes, PcmDecodeInfo,
+    ReplayGainSynthesisInfo)."""
+    dec = Decoder(2, 16, 44100, 4096, device=device)
+    try:
+        dec.index_files([bytes(b) for b in blobs])
+        return dec.decode_pcm_files_replaygain(spec=spec, per_file=per_file, kind=kind, **opts)
+    finally:
+        dec.close()
+
+
+def debug_tanh(x, device=0):
+    """fb200_debug_tanh: the device restatement of the host libm's tanh over x (float64)."""
+    x = np.ascontiguousarray(x, dtype=np.float64)
+    y = np.empty_like(x)
+    _check(lib().fb200_debug_tanh(x.ctypes.data, y.ctypes.data, x.size, device))
+    return y
+
+
+def debug_replaygain_synthesis(x, blocks, bps, scale, hard_limit, noise_shaping, first_draw=0, device=0):
+    """fb200_debug_replaygain_synthesis: apply_gain's val32 for int32 x [samples, channels] delivered in `blocks`."""
+    x = np.ascontiguousarray(x, dtype=np.int32)
+    b = np.ascontiguousarray(blocks, dtype=np.uint32)
+    out = np.empty_like(x)
+    _check(lib().fb200_debug_replaygain_synthesis(device, x.ctypes.data, x.shape[1], x.shape[0], b.ctypes.data, b.size, bps, scale,
+                                                  1 if hard_limit else 0, noise_shaping, first_draw, out.ctypes.data))
+    return out
 
 
 def preset(channels, bits_per_sample, sample_rate, compression_level, blocksize=0, **overrides):
@@ -1142,6 +1222,39 @@ class Decoder:
         if not (rc == -4 and out_capacity == 0):
             _check(rc)
         return list(infos[:n]), total.value
+
+    def decode_pcm_files_replaygain(self, spec=None, per_file=False, kind="wave", subformat=None, md5=True, ranges=None, channel_map_none=False):
+        """flac -d --apply-replaygain-which-is-not-lossless[=SPEC] over the files of the last index_files: decode_pcm_files with
+        ReplayGain applied where the tool applies it (spec None: the option without '='). per_file as decode_pcm_files_replaygain.
+        Returns [(bytes, PcmDecodeInfo, ReplayGainSynthesisInfo)]."""
+        opt, arr, nr, n = self._pcm_args(kind, subformat, md5, ranges, channel_map_none)
+        rg = spec if isinstance(spec, ReplayGainSynthesis) else replaygain_synthesis(spec, per_file)
+        infos = (PcmDecodeInfo * max(n, 1))()
+        rginfos = (ReplayGainSynthesisInfo * max(n, 1))()
+        total = C.c_uint64(0)
+        rc = lib().fb200_decode_pcm_files_replaygain_host(self._h, C.byref(opt), C.byref(rg), arr, nr, None, 0, C.byref(total), infos, rginfos)
+        if rc not in (FB200_OK, -4):
+            _check(rc)
+        out = np.empty(max(total.value, 1), dtype=np.uint8)
+        if rc != FB200_OK:
+            _check(lib().fb200_decode_pcm_files_replaygain_host(self._h, C.byref(opt), C.byref(rg), arr, nr, out.ctypes.data, total.value, C.byref(total),
+                                                                infos, rginfos))
+        return [(out[int(i.offset):int(i.offset) + int(i.bytes)].tobytes(), i, r) for i, r in zip(infos[:n], rginfos[:n])]
+
+    def decode_pcm_files_replaygain_device(self, d_out_ptr, out_capacity, spec=None, per_file=False, kind="wave", subformat=None, md5=True,
+                                           ranges=None, channel_map_none=False, stream=0):
+        """decode_pcm_files_replaygain into device memory (container i at infos[i].offset). out_capacity 0 sizes the call. Returns
+        after completion with ([PcmDecodeInfo], [ReplayGainSynthesisInfo], total bytes)."""
+        opt, arr, nr, n = self._pcm_args(kind, subformat, md5, ranges, channel_map_none)
+        rg = spec if isinstance(spec, ReplayGainSynthesis) else replaygain_synthesis(spec, per_file)
+        infos = (PcmDecodeInfo * max(n, 1))()
+        rginfos = (ReplayGainSynthesisInfo * max(n, 1))()
+        total = C.c_uint64(0)
+        rc = lib().fb200_decode_pcm_files_replaygain_device(self._h, C.byref(opt), C.byref(rg), arr, nr, d_out_ptr, out_capacity, C.byref(total), infos,
+                                                            rginfos, C.c_void_p(stream))
+        if not (rc == -4 and out_capacity == 0):
+            _check(rc)
+        return list(infos[:n]), list(rginfos[:n]), total.value
 
     def _add_rg_args(self, files, albums, scan, whole_files):
         files = np.ascontiguousarray(files, dtype=np.uint32)

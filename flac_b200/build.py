@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = [os.path.join(HERE, "csrc", f) for f in ("encoder.cu", "general_kernels.cu", "autoc_kernel.cu", "search_kernel.cu", "emit_kernel.cu",
                                               "tiled_kernels.cu", "files_kernels.cu", "md5_kernel.cu", "files_decode_kernels.cu", "flac_parse.cu", "decoder.cu",
                                               "stream_api.cu", "flac_metadata.cu", "pcm_container.cu", "replaygain_kernel.cu",
-                                              "reencode.cu", "add_replaygain.cu")]
+                                              "reencode.cu", "add_replaygain.cu", "replaygain_synthesis.cu")]
 OBJ_DIR = os.path.join(HERE, "csrc", "_obj")
 HDR = sorted(glob.glob(os.path.join(HERE, "csrc", "*.h")) + glob.glob(os.path.join(HERE, "csrc", "*.cuh"))) + [
     os.path.join(HERE, "..", "include", "flac_b200.h"), os.path.join(HERE, "..", "include", "flac_b200_stream.h")]

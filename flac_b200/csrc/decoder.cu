@@ -81,6 +81,10 @@ struct fb200_decoder {
 	std::vector<uint32_t> files_pos;                 // ... and its place in files_order (~0u: not OK)
 	uint8_t *d_pwork = nullptr;                      // ... and k_pcm_pack's plan: segments, their containers, containers, headers
 	size_t d_pwork_cap = 0;
+	uint8_t *d_keep = nullptr;                       // fb200_decode_pcm_files_replaygain_*: every candidate's frame bytes and place
+	size_t d_keep_cap = 0;
+	uint8_t *d_rgswork = nullptr;                    // ... and k_rg_synth's plan
+	size_t d_rgswork_cap = 0;
 };
 
 // device buffer of at least `need` bytes (contents not kept)
@@ -178,6 +182,7 @@ void fb200_decoder_destroy(fb200_decoder *d)
 	for(cudaEvent_t ev : d->ev_done) cudaEventDestroy(ev);
 	cudaFree(d->d_packed);
 	cudaFree(d->d_fdata); cudaFree(d->d_findex); cudaFree(d->d_fwork); cudaFree(d->d_fslots); cudaFree(d->d_rwork); cudaFree(d->d_rcand); cudaFree(d->d_pwork);
+	cudaFree(d->d_keep); cudaFree(d->d_rgswork);
 	delete d;
 }
 
@@ -726,8 +731,10 @@ static int decode_files_run(fb200_decoder *d, const FilesRun &R, uint32_t *d_sta
 }
 
 // Decodes the resident batch into d_out (int32, total values, zeroed first). skip_bps: groups deeper than this are not decoded
-// (FB200_FILE_WIDTH). Returns after completion with files[] filled.
-static int decode_files_impl(fb200_decoder *d, int32_t *d_out, uint32_t skip_bps, int do_md5, fb200_file_decode_info *files, cudaStream_t st)
+// (FB200_FILE_WIDTH). Returns after completion with files[] filled. With kept, every candidate's place (FilePlace, indexed as the
+// resident index) is copied there too.
+static int decode_files_impl(fb200_decoder *d, int32_t *d_out, uint32_t skip_bps, int do_md5, fb200_file_decode_info *files, cudaStream_t st,
+                             std::vector<FilePlace> *kept = nullptr)
 {
 	const uint32_t nfiles = (uint32_t)d->files_info.size();
 	const FilesIndexLayout L(d->files_ncand, d->files_state0.size());
@@ -775,6 +782,11 @@ static int decode_files_impl(fb200_decoder *d, int32_t *d_out, uint32_t skip_bps
 	uint32_t *d_stat = reinterpret_cast<uint32_t *>(d->d_fwork + o_stat);
 	uint32_t *d_bytes = reinterpret_cast<uint32_t *>(d->d_fwork + o_bytes);
 	FilePlace *d_place = reinterpret_cast<FilePlace *>(d->d_fwork + o_place);
+	const size_t k_bytes = align16((size_t)d->files_ncand * sizeof(FilePlace));
+	if(kept) {
+		if((rc = grow((void **)&d->d_keep, &d->d_keep_cap, k_bytes + (size_t)d->files_ncand * sizeof(uint32_t) + 16)) != FB200_OK) return rc;
+		if(d->files_ncand) FB_CUDA(cudaMemsetAsync(d->d_keep, 0, k_bytes, st));
+	}
 
 	if(!d->files_state0.empty())
 		FB_CUDA(cudaMemcpyAsync(d_states, d->files_state0.data(), d->files_state0.size() * sizeof(FileDecState), cudaMemcpyHostToDevice, st));
@@ -786,7 +798,14 @@ static int decode_files_impl(fb200_decoder *d, int32_t *d_out, uint32_t skip_bps
 			continue;
 		}
 		const FilesRun R{&G, G.cand0, G.ncand, d->files_state0.data() + G.pos0, d_states + G.pos0, G.nfiles, d_begins, d_ends, d_cands};
-		if((rc = decode_files_run(d, R, d_stat, d_bytes, d_place, d_out, st)) != FB200_OK) return rc;
+		if(kept) rc = decode_files_run(d, R, d_stat, reinterpret_cast<uint32_t *>(d->d_keep + k_bytes), reinterpret_cast<FilePlace *>(d->d_keep), d_out, st,
+		                               nullptr, 0, true);
+		else rc = decode_files_run(d, R, d_stat, d_bytes, d_place, d_out, st);
+		if(rc != FB200_OK) return rc;
+	}
+	if(kept) {
+		kept->resize(d->files_ncand);
+		if(d->files_ncand) FB_CUDA(cudaMemcpyAsync(kept->data(), d->d_keep, (size_t)d->files_ncand * sizeof(FilePlace), cudaMemcpyDeviceToHost, st));
 	}
 	uint8_t *d_digests = d->d_fwork + o_md5;
 	for(int w = 1; w <= 4; w++)
@@ -897,9 +916,11 @@ static int ranges_layout(const fb200_decoder *d, const fb200_sample_range *range
 
 // Decodes the ranges whose layout ranges_layout() gave into d_out (int32, total values, zeroed first). Returns after completion
 // with nframes / samples_missing / candidates of info[] filled (and errors[r], when given, with range r's damaged stretches +
-// overlapping frames). The resident index is only read.
+// overlapping frames). The resident index is only read. With kept, the place of every candidate selected for range r is copied to
+// (*kept)[kept0[r] ..], info[r].candidates of them.
 static int decode_files_ranges_impl(fb200_decoder *d, const fb200_sample_range *ranges, uint32_t nranges, int32_t *d_out, uint64_t total,
-                                    fb200_range_decode_info *info, cudaStream_t st, uint32_t *errors = nullptr)
+                                    fb200_range_decode_info *info, cudaStream_t st, uint32_t *errors = nullptr, std::vector<FilePlace> *kept = nullptr,
+                                    std::vector<uint64_t> *kept0 = nullptr)
 {
 	const uint32_t nfiles = (uint32_t)d->files_info.size(), ngroups = (uint32_t)d->files_groups.size();
 	const FilesIndexLayout L(d->files_ncand, d->files_state0.size());
@@ -1000,12 +1021,26 @@ static int decode_files_ranges_impl(fb200_decoder *d, const fb200_sample_range *
 	uint32_t *d_stat = reinterpret_cast<uint32_t *>(d->d_fwork + o_stat);
 	uint32_t *d_bytes = reinterpret_cast<uint32_t *>(d->d_fwork + o_bytes);
 	FilePlace *d_place = reinterpret_cast<FilePlace *>(d->d_fwork + o_place);
+	const size_t k_bytes = align16((size_t)nsel * sizeof(FilePlace));
+	if(kept) {
+		if((rc = grow((void **)&d->d_keep, &d->d_keep_cap, k_bytes + (size_t)nsel * sizeof(uint32_t) + 16)) != FB200_OK) return rc;
+		if(nsel) FB_CUDA(cudaMemsetAsync(d->d_keep, 0, k_bytes, st));
+	}
 	for(uint32_t g = 0; g < ngroups; g++) {
 		const uint32_t a = gfirst[g], b = gfirst[g + 1];
 		if(a == b) continue;
 		const uint64_t c0 = dst[a], c1 = b < n ? dst[b] : nsel;
 		const FilesRun R{&d->files_groups[g], c0, c1 - c0, states.data() + a, d_states + a, b - a, d_rbeg, d_rend, d_rcands};
-		if((rc = decode_files_run(d, R, d_stat, d_bytes, d_place, d_out, st)) != FB200_OK) return rc;
+		if(kept) rc = decode_files_run(d, R, d_stat, reinterpret_cast<uint32_t *>(d->d_keep + k_bytes), reinterpret_cast<FilePlace *>(d->d_keep), d_out, st,
+		                               nullptr, 0, true);
+		else rc = decode_files_run(d, R, d_stat, d_bytes, d_place, d_out, st);
+		if(rc != FB200_OK) return rc;
+	}
+	if(kept) {
+		kept->resize(nsel);
+		kept0->assign(nranges, 0);
+		for(uint32_t i = 0; i < n; i++) (*kept0)[order[i]] = dst[i];
+		if(nsel) FB_CUDA(cudaMemcpyAsync(kept->data(), d->d_keep, (size_t)nsel * sizeof(FilePlace), cudaMemcpyDeviceToHost, st));
 	}
 	FB_CUDA(cudaGetLastError());
 	FB_CUDA(cudaMemcpyAsync(states.data(), d_states, n * sizeof(FileDecState), cudaMemcpyDeviceToHost, st));
@@ -1066,10 +1101,36 @@ int fb200_decode_files_ranges_host(fb200_decoder *d, const fb200_sample_range *r
 }
 
 // ---------------------------------------------------------------- the resident batch as container files (flac -d)
+// The delivered blocks of one container (the accepted frames' parts inside it, in order, as FilePlace entries of its values from
+// value v0 on) as k_rg_synth takes them: appended to blocks, gaps filled so that they tile [0, ns). Returns the samples the tool
+// writes before its first error: the blocks before the first sample no frame covers.
+static uint64_t rgs_blocks(const FilePlace *place, uint64_t nplace, uint64_t v0, uint32_t C, uint64_t ns, std::vector<RgsBlock> &blocks)
+{
+	uint64_t pos = 0, delivered = 0;
+	bool whole = true;
+	for(uint64_t k = 0; k < nplace; k++) {
+		const FilePlace &q = place[k];
+		if(q.n == 0) continue;
+		const uint64_t s = (q.dst - v0) / C, m = q.n / C;
+		if(s > pos) {
+			blocks.push_back(RgsBlock{pos, s - pos});
+			whole = false;
+		}
+		blocks.push_back(RgsBlock{s, m});
+		pos = s + m;
+		if(whole) delivered = pos;
+	}
+	if(pos < ns) blocks.push_back(RgsBlock{pos, ns - pos});
+	return delivered;
+}
+
 // Sizes every container on the host, decodes into the int32 scratch by the whole-file or the ranged path, then packs every
-// container with one k_pcm_pack launch into `out` (device memory; the caller's with _device, d_packed with _host).
+// container with one k_pcm_pack launch into `out` (device memory; the caller's with _device, d_packed with _host). With rg, the
+// containers the tool applies ReplayGain to get apply_gain's values (k_rg_synth, in place in the scratch) and are packed with
+// shift 0; rginfo[n] receives the decisions and draw positions.
 static int decode_pcm_files(fb200_decoder *d, const fb200_pcm_decode_options *opt, const fb200_sample_range *ranges, uint32_t nranges, bool host,
-                            uint8_t *out, uint64_t out_capacity, uint64_t *total_bytes, fb200_pcm_decode_info *info, cudaStream_t st)
+                            uint8_t *out, uint64_t out_capacity, uint64_t *total_bytes, fb200_pcm_decode_info *info, cudaStream_t st,
+                            const fb200_replaygain_synthesis *rg = nullptr, fb200_replaygain_synthesis_info *rginfo = nullptr)
 {
 	if(!d || !total_bytes || !info) return FB200_ERR_INVALID;
 	if(!pcm_decode_options_ok(opt)) return FB200_ERR_INVALID;
@@ -1107,6 +1168,27 @@ static int decode_pcm_files(fb200_decoder *d, const fb200_pcm_decode_options *op
 		off += I.bytes;
 	}
 	*total_bytes = off;
+	if(rg) {
+		// the tool's decision per container, from its file's metadata (each file read once)
+		std::map<uint32_t, fb200_replaygain_synthesis_info> seen;
+		FB_CUDA(cudaSetDevice(d->device));
+		for(uint32_t i = 0; i < n; i++) {
+			fb200_replaygain_synthesis_info &R = rginfo[i];
+			memset(&R, 0, sizeof R);
+			R.status = FB200_RGS_NOT_DECODED;
+			if(info[i].status != FB200_FILE_OK) continue;
+			const uint32_t f = whole ? i : ranges[i].file;
+			auto it = seen.find(f);
+			if(it == seen.end()) {
+				std::vector<uint8_t> meta;
+				if((rc = decoder_file_metadata(d, f, &meta)) != FB200_OK) return rc;
+				fb200_replaygain_synthesis_info D;
+				rgs_decide(meta.data(), meta.size(), d->files_info[f].bits_per_sample, *rg, &D);
+				it = seen.emplace(f, D).first;
+			}
+			R = it->second;
+		}
+	}
 	if(out_capacity < off) { set_error("output holds %llu bytes, the containers need %llu", (unsigned long long)out_capacity, (unsigned long long)off); return FB200_ERR_OUTPUT_TOO_SMALL; }
 	if(!out && off) { set_error("out is NULL"); return FB200_ERR_INVALID; }
 	FB_CUDA(cudaSetDevice(d->device));
@@ -1120,13 +1202,57 @@ static int decode_pcm_files(fb200_decoder *d, const fb200_pcm_decode_options *op
 	}
 	std::vector<fb200_file_decode_info> finfo(whole ? n : 0);
 	std::vector<uint32_t> rerr(whole ? 0 : n, 0);
-	if(whole) rc = decode_files_impl(d, d->d_pcm, 24, opt->md5 ? 1 : 0, finfo.data(), st);
+	bool applied = false;
+	for(uint32_t i = 0; rg && i < n; i++) applied |= info[i].status == FB200_FILE_OK && rginfo[i].status == FB200_RGS_APPLIED;
+	std::vector<FilePlace> kept;
+	std::vector<uint64_t> kept0;
+	const bool keep = applied && rg->noise_shaping != 0;
+	if(whole) rc = decode_files_impl(d, d->d_pcm, 24, opt->md5 ? 1 : 0, finfo.data(), st, keep ? &kept : nullptr);
 	else {
 		for(uint32_t i = 0; i < n; i++)
 			if(info[i].status != FB200_FILE_OK) rinfo[i].status = info[i].status;  // not decoded
-		rc = decode_files_ranges_impl(d, ranges, nranges, d->d_pcm, rvalues, rinfo.data(), st, rerr.data());
+		rc = decode_files_ranges_impl(d, ranges, nranges, d->d_pcm, rvalues, rinfo.data(), st, rerr.data(), keep ? &kept : nullptr, keep ? &kept0 : nullptr);
 	}
 	if(rc != FB200_OK) return rc;
+
+	// ---- ReplayGain: the plan of k_rg_synth over every container the tool applies gain to
+	if(applied) {
+		RgsPlan plan;
+		uint64_t draw = 0;  // the generator's position, running on over the containers of one invocation
+		unsigned long long rg_items = 0;
+		for(uint32_t i = 0; i < n; i++) {
+			fb200_replaygain_synthesis_info &R = rginfo[i];
+			if(info[i].status != FB200_FILE_OK || R.status != FB200_RGS_APPLIED) continue;
+			const uint32_t C = info[i].channels;
+			const uint64_t ns = info[i].samples, v0 = whole ? finfo[i].first_value : rinfo[i].first_value;
+			const RgsParam P = rgs_param(info[i].bits_per_sample, R.scale, rg->limiter == FB200_RGS_LIMIT_HARD, rg->noise_shaping);
+			R.first_draw = whole && !rg->per_file ? draw : 0;
+			if(ns == 0) continue;
+			if(rg->noise_shaping == 0) {
+				plan.segs.push_back(RgsSeg{v0, ns * C, rg_items, P});
+				rg_items += (ns * C + 1023) / 1024;
+				continue;
+			}
+			const FilePlace *place;
+			uint64_t nplace;
+			if(whole) {
+				const FileDecState &S = d->files_state0[d->files_pos[i]];
+				place = kept.data() + S.cand0;
+				nplace = S.ncand;
+			}
+			else {
+				place = kept.data() + (kept0.empty() ? 0 : kept0[i]);
+				nplace = kept.empty() ? 0 : rinfo[i].candidates;
+			}
+			const uint32_t b0 = (uint32_t)plan.blocks.size();
+			const uint64_t delivered = rgs_blocks(place, nplace, v0, C, ns, plan.blocks);
+			R.draws = 2ull * C * delivered;
+			draw = R.first_draw + R.draws;
+			for(uint32_t c = 0; c < C; c++)
+				plan.chains.push_back(RgsChain{v0, ns, R.first_draw, C, c, b0, (uint32_t)plan.blocks.size() - b0, P});
+		}
+		if((rc = rgs_run(plan, rg->noise_shaping, d->d_pcm, st, &d->d_rgswork, &d->d_rgswork_cap, &d->launches)) != FB200_OK) return rc;
+	}
 
 	// ---- the pack plan: one segment per container with values, one PcmPackDev per container, the headers back to back
 	std::vector<FileSeg> segs;
@@ -1156,7 +1282,7 @@ static int decode_pcm_files(fb200_decoder *d, const fb200_pcm_decode_options *op
 		P.out = I.offset; P.blob = blob.size(); P.data = h.data_bytes; P.hlen = h.length; P.pad = (uint32_t)h.pad; P.bytes = B;
 		P.big = opt->kind == FB200_PCM_AIFF || (opt->kind == FB200_PCM_AIFF_C && opt->subformat == FB200_PCM_SUB_AIFF_C_NONE);
 		P.is_unsigned = opt->kind != FB200_PCM_AIFF && opt->kind != FB200_PCM_AIFF_C && I.bits_per_sample <= 8;
-		P.shift = h.container_bits - I.bits_per_sample;
+		P.shift = rg && rginfo[i].status == FB200_RGS_APPLIED ? 0 : h.container_bits - I.bits_per_sample;  // apply_gain's values are at the target width
 		const uint64_t nv = I.samples * I.channels;
 		if(nv) {
 			segs.push_back(FileSeg{src, I.offset + h.length, nv, items});
@@ -1204,6 +1330,25 @@ int fb200_decode_pcm_files_device(fb200_decoder *d, const fb200_pcm_decode_optio
                                   uint8_t *d_out, uint64_t out_capacity, uint64_t *total_bytes, fb200_pcm_decode_info *info, void *cuda_stream)
 {
 	return decode_pcm_files(d, opt, ranges, nranges, false, d_out, out_capacity, total_bytes, info, (cudaStream_t)cuda_stream);
+}
+
+int fb200_decode_pcm_files_replaygain_host(fb200_decoder *d, const fb200_pcm_decode_options *opt, const fb200_replaygain_synthesis *rg,
+                                           const fb200_sample_range *ranges, uint32_t nranges, uint8_t *out, uint64_t out_capacity,
+                                           uint64_t *total_bytes, fb200_pcm_decode_info *info, fb200_replaygain_synthesis_info *rginfo)
+{
+	if(!d || !rginfo) return FB200_ERR_INVALID;
+	if(!rgs_spec_ok(rg)) return FB200_ERR_INVALID;
+	return decode_pcm_files(d, opt, ranges, nranges, true, out, out_capacity, total_bytes, info, d->stream, rg, rginfo);
+}
+
+int fb200_decode_pcm_files_replaygain_device(fb200_decoder *d, const fb200_pcm_decode_options *opt, const fb200_replaygain_synthesis *rg,
+                                             const fb200_sample_range *ranges, uint32_t nranges, uint8_t *d_out, uint64_t out_capacity,
+                                             uint64_t *total_bytes, fb200_pcm_decode_info *info, fb200_replaygain_synthesis_info *rginfo,
+                                             void *cuda_stream)
+{
+	if(!d || !rginfo) return FB200_ERR_INVALID;
+	if(!rgs_spec_ok(rg)) return FB200_ERR_INVALID;
+	return decode_pcm_files(d, opt, ranges, nranges, false, d_out, out_capacity, total_bytes, info, (cudaStream_t)cuda_stream, rg, rginfo);
 }
 
 }  // extern "C"

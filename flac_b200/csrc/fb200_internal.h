@@ -447,6 +447,30 @@ struct RgFramesOut { unsigned long long nwin; uint32_t peak, ok; };
 void launch_replaygain_frames(const int32_t *pcm, const RgFramesFileDev *files, int nfiles, const FilePlace *place, const unsigned long long *begins,
                               const uint32_t *bytes, const FileDecCand *cands, const FileDecState *states, double *v, RgFramesOut *out, cudaStream_t st);
 
+// ---- ReplayGain synthesis (replaygain_synthesis.cu): flac -d --apply-replaygain-which-is-not-lossless
+// The constants of apply_gain for one container: multi_scale, the dither context's Add / Mask / Dither (from the stream's bits),
+// conv_shift and the clip factor (from the target width), and whether the hard limiter runs.
+struct RgsParam { double multi, add; unsigned long long mask; long long clip; float dither; int conv_shift, hard, pad; };
+RgsParam rgs_param(uint32_t bps, double scale, bool hard, uint32_t shaping);
+// No shaping: values [v0, v0 + n) of the int32 scratch, CTAs from item0 on
+struct RgsSeg { unsigned long long v0, n, item0; RgsParam P; };
+// A delivered block (what the tool's write callback receives): samples [s, s + n) from the container's first sample
+struct RgsBlock { unsigned long long s, n; };
+// With shaping: channel c of a container of C channels and ns samples whose first value is v0; its blocks [b0, b0 + nb) tile
+// [0, ns); draw0 is the generator's position at the container's first sample
+struct RgsChain { unsigned long long v0, ns, draw0; uint32_t C, c, b0, nb; RgsParam P; };
+struct RgsPlan {
+	std::vector<RgsSeg> segs;
+	std::vector<RgsChain> chains;
+	std::vector<RgsBlock> blocks;
+};
+// Applies the plan to the int32 scratch in place (val32 per value): k_rg_synth0 for segs, k_rg_synth<shaping> for chains. work is
+// grown as needed.
+int rgs_run(const RgsPlan &plan, uint32_t shaping, int32_t *pcm, cudaStream_t st, uint8_t **work, size_t *work_cap, uint64_t *launches);
+// The tool's decision for one .flac file (its bytes) of a bps-bit stream; first_draw and draws are left 0
+void rgs_decide(const uint8_t *p, size_t n, uint32_t bps, const fb200_replaygain_synthesis &rg, fb200_replaygain_synthesis_info *info);
+bool rgs_spec_ok(const fb200_replaygain_synthesis *rg);  // sets the error when not
+
 // encoder.cu: the verify records of the last call, spread over nlisted entries (records[i] goes to entry at[i], the rest OK)
 void encoder_spread_verify(fb200_encoder *e, const std::vector<uint32_t> &at, uint32_t nlisted);
 int encoder_device(const fb200_encoder *e);

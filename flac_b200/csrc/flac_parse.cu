@@ -153,22 +153,54 @@ static bool vorbis_channel_mask(const uint8_t *b, uint32_t len, uint32_t *mask)
 	return false;
 }
 
-uint32_t channel_mask_tag(const uint8_t *p, size_t n)
+void for_each_vorbis_comment(const uint8_t *p, size_t n, const std::function<void(const uint8_t *, uint32_t)> &fn)
 {
-	uint32_t mask = 0;
 	size_t pos = 0;
 	if(n >= 10 && memcmp(p, "ID3", 3) == 0) pos = id3v2_tag_bytes(p);
-	if(pos > n || n - pos < 4 || memcmp(p + pos, "fLaC", 4) != 0) return 0;
+	if(pos > n || n - pos < 4 || memcmp(p + pos, "fLaC", 4) != 0) return;
 	pos += 4;
 	for(bool last = false; !last;) {
 		if(n - pos < 4) break;
 		const MetaBlockHeader h = metadata_block_header(p + pos);
 		last = h.last;
 		if(n - pos - 4 < h.length) break;
-		if(h.type == FLAC__METADATA_TYPE_VORBIS_COMMENT) vorbis_channel_mask(p + pos + 4, h.length, &mask);
+		if(h.type == FLAC__METADATA_TYPE_VORBIS_COMMENT) fn(p + pos + 4, h.length);
 		pos += 4 + (size_t)h.length;
 	}
+}
+
+uint32_t channel_mask_tag(const uint8_t *p, size_t n)
+{
+	uint32_t mask = 0;
+	for_each_vorbis_comment(p, n, [&](const uint8_t *b, uint32_t len) { vorbis_channel_mask(b, len, &mask); });
 	return mask;
+}
+
+bool vorbis_entries(const uint8_t *b, uint32_t len, std::vector<std::string> *ent)
+{
+	auto le32 = [](const uint8_t *q) { return (uint32_t)q[0] | (uint32_t)q[1] << 8 | (uint32_t)q[2] << 16 | (uint32_t)q[3] << 24; };
+	ent->clear();
+	if(len < 8) return false;
+	uint32_t left = len - 4;
+	const uint32_t vendor = le32(b);
+	if(left < vendor) return false;
+	left -= vendor;
+	if(left < 4) return false;
+	left -= 4;
+	const uint8_t *q = b + 4 + vendor;
+	const uint32_t num = le32(q);
+	q += 4;
+	if(num > 100000) return false;
+	for(uint32_t i = 0; i < num; i++) {
+		if(left < 4) break;  // the block ends here: the entries read so far stand, unless bytes are left over (below)
+		left -= 4;
+		const uint32_t el = le32(q);
+		if(left < el) return false;
+		left -= el;
+		ent->emplace_back(reinterpret_cast<const char *>(q + 4), el);
+		q += 4 + el;
+	}
+	return left == 0;
 }
 
 }  // namespace fb200

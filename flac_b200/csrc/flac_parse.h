@@ -5,6 +5,10 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <functional>
+#include <string>
+#include <vector>
+
 #include "../../include/flac_b200_stream.h"
 
 namespace fb200 {
@@ -47,5 +51,15 @@ bool walk_metadata(const uint8_t *p, size_t n, FLAC__StreamMetadata_StreamInfo &
 // than the name and its value is "0x" (any case) followed by what sscanf("%x") reads; a later block's valid tag overrides an
 // earlier one. 0 when no block has one.
 uint32_t channel_mask_tag(const uint8_t *p, size_t n);
+
+// Calls fn(body, length) for every VORBIS_COMMENT block of a .flac file held whole in memory, in order (optional ID3v2 tag,
+// "fLaC", then the blocks up to the last one or the first that runs past the file).
+void for_each_vorbis_comment(const uint8_t *p, size_t n, const std::function<void(const uint8_t *, uint32_t)> &fn);
+
+// The entries of one VORBIS_COMMENT body as read_metadata_vorbiscomment_ (stream_decoder.c:2020-2125) keeps them: each its raw
+// bytes at its full length (embedded NULs included). Returns false where libFLAC fails the block (the metadata callback then
+// never sees it): the vendor string or an entry running past the block, more than 100000 entries, or bytes left after the last
+// entry read. When the block ends exactly between entries, the entries read so far are kept.
+bool vorbis_entries(const uint8_t *b, uint32_t len, std::vector<std::string> *ent);
 
 }  // namespace fb200

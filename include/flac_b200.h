@@ -820,6 +820,65 @@ int fb200_decode_pcm_files_device(fb200_decoder *dec, const fb200_pcm_decode_opt
                                   const fb200_sample_range *ranges, uint32_t nranges,
                                   uint8_t *d_out, uint64_t out_capacity, uint64_t *total_bytes, fb200_pcm_decode_info *info,
                                   void *cuda_stream);
+/* ---- the same containers with ReplayGain applied (flac -d --apply-replaygain-which-is-not-lossless[=SPEC]) ----
+ * fb200_decode_pcm_files_replaygain_* write what fb200_decode_pcm_files_* write (same lengths, headers, pad bytes, statuses,
+ * tool_ok and MD5 of the decoded samples before gain), except that the samples of each container the tool applies gain to are
+ * those of FLAC__replaygain_synthesis__apply_gain (src/share/replaygain_synthesis/replaygain_synthesis.c): scaled, optionally
+ * hard-limited (glibc tanh restated bit for bit), re-quantised to the container's width, with noise-shaped triangular dither
+ * for noise_shaping 1-3. The decision per file follows the tool's metadata callback (decode.c:1775-1820,
+ * grabbag/replaygain.c:582-669): names matched without case, values read by strtod in the C locale from the first
+ * min(31, length - 1) characters after '=' (parse_double_'s safe_strncpy drops the last one), a negative peak fails the pair, a
+ * failed pair retries the other mode, and the last VORBIS_COMMENT block decides. Then bits per sample outside 4-24 is BPS,
+ * |gain| > 90 is GAIN, no usable pair is NO_TAGS, and the container is decoded plainly.
+ *
+ * The dither generator of the tool (random_int_) is process-global: its state runs on from file to file of one invocation.
+ * Whole files with per_file 0 reproduce one invocation over the listed files in order; per_file 1 and every range reproduce one
+ * invocation per container. A file draws 2 x channels numbers per sample the tool writes before its first decode error (the
+ * write callback aborts there); rginfo[i].first_draw / draws say where each container's draws lie. The engine still writes a
+ * damaged file in full with tool_ok 0, its samples after the error dithered with draws that follow on. Known difference: the
+ * first error is taken to be the first sample no accepted frame covers, so a damaged stretch that loses no samples (junk
+ * between frames) does not end a file's draws as it ends the tool's. */
+enum { FB200_RGS_LIMIT_NONE = 0, FB200_RGS_LIMIT_PEAK = 1, FB200_RGS_LIMIT_HARD = 2 };
+typedef struct {
+	double   preamp;         /* dB */
+	uint32_t album;          /* 1: album gain and peak (falls back to track); 0: track (falls back to album) */
+	uint32_t limiter;        /* FB200_RGS_LIMIT_* */
+	uint32_t noise_shaping;  /* 0: no dither; 1-3: low / medium / high (triangular dither, 16-tap shaping filter) */
+	uint32_t per_file;       /* whole files: 0 = the list is one invocation, 1 = one invocation per file; ranges: always per range */
+} fb200_replaygain_synthesis;
+/* The tool's parse of SPEC (main.c:767-790); spec NULL: the option without '=' (album, hard limiter, low shaping, preamp 0).
+ * FB200_ERR_INVALID where the tool prints a usage error. per_file is set to 0. */
+int fb200_replaygain_synthesis_parse(const char *spec, fb200_replaygain_synthesis *rg);
+enum { FB200_RGS_APPLIED = 0, FB200_RGS_NO_TAGS = 1, FB200_RGS_BPS = 2, FB200_RGS_GAIN = 3, FB200_RGS_NOT_DECODED = 4 };
+typedef struct {
+	uint32_t status;                 /* FB200_RGS_*: the tool's decision; not APPLIED = the plain decode's bytes */
+	uint32_t album_used;             /* which tag pair gave gain and peak after the fallback */
+	double   reference, gain, peak;  /* as parsed */
+	double   scale;                  /* grabbag__replaygain_compute_scale_factor */
+	uint64_t first_draw, draws;      /* the generator's position at the container's first sample, and the draws the tool makes for it */
+} fb200_replaygain_synthesis_info;
+/* Device-free: the decision and the scale for one .flac from its metadata; first_draw and draws are left 0. */
+int fb200_replaygain_synthesis_file(const uint8_t *file, uint64_t nbytes, const fb200_replaygain_synthesis *rg,
+                                    fb200_replaygain_synthesis_info *info);
+/* As fb200_decode_pcm_files_host / _device, with rginfo[n] (one per container) filled before the capacity check. Containers
+ * that are not decoded get FB200_RGS_NOT_DECODED. One k_rg_synth launch per call (two when both shaping 0 and 1-3 would run,
+ * which one spec never asks for), whatever the number of files. */
+int fb200_decode_pcm_files_replaygain_host(fb200_decoder *dec, const fb200_pcm_decode_options *opt, const fb200_replaygain_synthesis *rg,
+                                           const fb200_sample_range *ranges, uint32_t nranges, uint8_t *out, uint64_t out_capacity,
+                                           uint64_t *total_bytes, fb200_pcm_decode_info *info, fb200_replaygain_synthesis_info *rginfo);
+int fb200_decode_pcm_files_replaygain_device(fb200_decoder *dec, const fb200_pcm_decode_options *opt, const fb200_replaygain_synthesis *rg,
+                                             const fb200_sample_range *ranges, uint32_t nranges, uint8_t *d_out, uint64_t out_capacity,
+                                             uint64_t *total_bytes, fb200_pcm_decode_info *info, fb200_replaygain_synthesis_info *rginfo,
+                                             void *cuda_stream);
+/* Debug: y[i] = the device restatement of the host libm's tanh(x[i]) (the hard limiter's). */
+int fb200_debug_tanh(const double *x, double *y, uint32_t n, int device);
+/* Debug: apply_gain on constructed input. `in`: channels x samples int32 values, interleaved; `blocks`: nblocks lengths summing to
+ * samples, the lengths the write callback would receive; the generator starts at draw first_draw. bps 4-24 is the source
+ * width; the target is the container's, 8 x ((bps + 7) / 8). scale, limiter (hard or not) and noise_shaping as the tool uses them.
+ * out: the val32 of every value (interleaved), before byte packing. */
+int fb200_debug_replaygain_synthesis(int device, const int32_t *in, uint32_t channels, uint64_t samples, const uint32_t *blocks, uint32_t nblocks,
+                                     uint32_t bps, double scale, uint32_t hard_limit, uint32_t noise_shaping, uint64_t first_draw, int32_t *out);
+
 /* Device-free: the header the tool writes for these facts into out[0 .. *length), *length being where the data begins.
  * channel_mask: the tag's value (0: none; the default for the channel count then applies), ignored with channel_map_none.
  * channels 1-8, bits_per_sample 4-32, else FB200_ERR_INVALID; FB200_ERR_UNSUPPORTED (*length 0) where the tool refuses the
