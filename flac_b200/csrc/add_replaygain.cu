@@ -10,6 +10,7 @@
 #include <map>
 
 #include "fb200_internal.h"
+#include "flac_metadata.h"
 #include "flac_parse.h"
 
 extern "C" const char *FLAC__VENDOR_STRING;
@@ -17,13 +18,6 @@ extern "C" const char *FLAC__VENDOR_STRING;
 namespace fb200 {
 
 namespace {
-
-uint32_t le32(const uint8_t *p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
-
-void put_le32(std::vector<uint8_t> &o, uint32_t v)
-{
-	for(int i = 0; i < 4; i++) o.push_back((uint8_t)(v >> (8 * i)));
-}
 
 // ---- the metadata chain (src/libFLAC/metadata_iterators.c)
 
@@ -37,52 +31,10 @@ struct ChainBlock {
 	std::vector<std::string> ent;
 };
 
-// read_metadata_block_data_vorbis_comment_cb_: the vendor and every entry must fit the block (else BAD_METADATA); a block that ends
-// after the vendor string has no entries; bytes after the last entry are skipped.
-bool read_vorbis_comment(const uint8_t *p, uint64_t n, ChainBlock *b)
-{
-	if(n < 4 || n - 4 < le32(p)) return false;
-	b->vendor.assign(reinterpret_cast<const char *>(p + 4), le32(p));
-	uint64_t pos = 4 + (uint64_t)le32(p);
-	if(n - pos < 4) return true;
-	const uint32_t count = le32(p + pos);
-	pos += 4;
-	if(count > (n - pos) / 4) return false;
-	for(uint32_t i = 0; i < count; i++) {
-		if(n - pos < 4) return false;
-		const uint32_t l = le32(p + pos);
-		pos += 4;
-		if(n - pos < l) return false;
-		b->ent.emplace_back(reinterpret_cast<const char *>(p + pos), l);
-		pos += l;
-	}
-	return true;
-}
-
-// A CUESHEET whose body is exactly its fields, with the reserved bits the writer zeroes cleared (format.c:158-191)
-bool read_cuesheet(std::vector<uint8_t> &b)
-{
-	const size_t n = b.size();
-	if(n < 396) return false;
-	b[136] &= 0x80;
-	memset(b.data() + 137, 0, 258);
-	size_t pos = 396;
-	for(uint32_t t = 0; t < b[395]; t++) {
-		if(n - pos < 36) return false;
-		b[pos + 21] &= 0xc0;
-		memset(b.data() + pos + 22, 0, 13);
-		const uint32_t nidx = b[pos + 35];
-		pos += 36;
-		if((n - pos) / 12 < nidx) return false;
-		for(uint32_t k = 0; k < nidx; k++, pos += 12) memset(b.data() + pos + 9, 0, 3);
-	}
-	return pos == n;
-}
-
 // A PICTURE whose body is exactly its fields (big-endian lengths)
 bool read_picture(const std::vector<uint8_t> &b)
 {
-	auto be32 = [&](size_t at) { return (uint32_t)b[at] << 24 | (uint32_t)b[at + 1] << 16 | (uint32_t)b[at + 2] << 8 | (uint32_t)b[at + 3]; };
+	auto be32 = [&](size_t at) { return be(b.data() + at, 4); };
 	const size_t n = b.size();
 	size_t pos = 4;
 	if(n < pos) return false;
@@ -101,19 +53,6 @@ uint64_t chain_length(const std::vector<ChainBlock> &L)
 	return n;
 }
 
-void vorbis_body(ChainBlock &b)
-{
-	b.body.clear();
-	put_le32(b.body, (uint32_t)b.vendor.size());
-	b.body.insert(b.body.end(), b.vendor.begin(), b.vendor.end());
-	put_le32(b.body, (uint32_t)b.ent.size());
-	for(const std::string &s : b.ent) {
-		put_le32(b.body, (uint32_t)s.size());
-		b.body.insert(b.body.end(), s.begin(), s.end());
-	}
-	b.length = b.body.size();
-}
-
 }  // namespace
 
 const char kBlockTooLong[] = "a metadata block is too long for its length field";  // the one refusal of the chain write
@@ -123,56 +62,41 @@ const char kBlockTooLong[] = "a metadata block is too long for its length field"
 const char *rg_rewrite_head(const uint8_t *m, uint64_t n, const float v[4], std::vector<uint8_t> *head, uint64_t *audio_in, bool *in_place)
 {
 	// FLAC__metadata_chain_read: an ID3v2 tag, "fLaC", the blocks (STREAMINFO first)
-	uint64_t pos = 0;
-	if(n >= 10 && memcmp(m, "ID3", 3) == 0) pos = id3v2_tag_bytes(m);
-	if(pos > n || n - pos < 4 || memcmp(m + pos, "fLaC", 4) != 0) return "not a FLAC file";
-	pos += 4;
-	const uint64_t prefix = pos;
+	const MetaRegion r = read_metadata_region(m, n);
+	if(r.end == MetaRegion::NO_MARKER) return "not a FLAC file";
 	std::vector<ChainBlock> L;
-	for(bool last = false; !last;) {
-		if(n - pos < 4) return "metadata runs past the file";
-		const MetaBlockHeader h = metadata_block_header(m + pos);
-		pos += 4;
-		if(n - pos < h.length) return "metadata runs past the file";
-		ChainBlock b{h.type, h.length, std::vector<uint8_t>(m + pos, m + pos + h.length), {}, {}};
-		pos += h.length;
-		last = h.last;
+	for(const MetaBlock &h : r.blocks) {
+		ChainBlock b{h.type, h.length, std::vector<uint8_t>(m + h.body, m + h.body + h.length), {}, {}};
 		switch(h.type) {
 			case 0: if(h.length != 34) return "STREAMINFO is not 34 bytes"; break;
 			case 1: b.body.clear(); break;
 			case 2: if(h.length < 4) return "APPLICATION block shorter than 4 bytes"; break;
 			case 3: if(h.length % 18) return "SEEKTABLE length is not a multiple of 18"; break;
-			case 4: if(!read_vorbis_comment(b.body.data(), h.length, &b)) return "VORBIS_COMMENT fields run past the block"; break;
-			case 5: if(!read_cuesheet(b.body)) return "CUESHEET body is not exactly its fields"; break;
+			case 4:
+				if(!read_metadata_block_data_vorbis_comment(b.body.data(), h.length, &b.vendor, &b.ent)) return "VORBIS_COMMENT fields run past the block";
+				break;
+			case 5: if(!cuesheet_zero_reserved(b.body.data(), b.body.size())) return "CUESHEET body is not exactly its fields"; break;
 			case 6: if(!read_picture(b.body)) return "PICTURE body is not exactly its fields"; break;
 			default: break;
 		}
 		L.push_back(std::move(b));
 	}
+	if(r.end == MetaRegion::SHORT) return "metadata runs past the file";
 	if(L.front().type != 0) return "first metadata block is not STREAMINFO";
 	const uint64_t initial = chain_length(L);
-	*audio_in = pos;
+	*audio_in = r.audio;
 
 	// the first VORBIS_COMMENT, or a new one after the last block; the three edits (grabbag__replaygain_store_to_vorbiscomment)
 	size_t vc = 0;
 	while(vc < L.size() && L[vc].type != 4) vc++;
-	if(vc == L.size()) {
-		L.push_back(ChainBlock{4, 0, {}, FLAC__VENDOR_STRING, {}});
-	}
-	static const char kRef[] = "REPLAYGAIN_REFERENCE_LOUDNESS", kTG[] = "REPLAYGAIN_TRACK_GAIN", kTP[] = "REPLAYGAIN_TRACK_PEAK",
-	                  kAG[] = "REPLAYGAIN_ALBUM_GAIN", kAP[] = "REPLAYGAIN_ALBUM_PEAK";
-	std::vector<std::string> &E = L[vc].ent;
-	vorbis_remove_matching(E, kRef);
-	E.push_back(rg_tag("%s=%2.1f dB", kRef, 89.0f));
-	vorbis_remove_matching(E, kTG);
-	vorbis_remove_matching(E, kTP);
-	E.push_back(rg_tag("%s=%+2.2f dB", kTG, v[0]));
-	E.push_back(rg_tag("%s=%1.8f", kTP, v[1]));
-	vorbis_remove_matching(E, kAG);
-	vorbis_remove_matching(E, kAP);
-	E.push_back(rg_tag("%s=%+2.2f dB", kAG, v[2]));
-	E.push_back(rg_tag("%s=%1.8f", kAP, v[3]));
-	vorbis_body(L[vc]);
+	if(vc == L.size()) L.push_back(ChainBlock{4, 0, {}, FLAC__VENDOR_STRING, {}});
+	ChainBlock &V = L[vc];
+	rg_edit(V.ent, RG_REFERENCE, 0.f, 0.f);
+	rg_edit(V.ent, RG_TRACK_GAIN, v[0], v[1]);
+	rg_edit(V.ent, RG_ALBUM_GAIN, v[2], v[3]);
+	V.body.clear();
+	put_vorbis_comment(V.body, V.vendor, V.ent);
+	V.length = V.body.size();
 
 	// FLAC__metadata_chain_sort_padding: every PADDING to the end, in order, then merged (4 + length per merged block)
 	{
@@ -186,31 +110,21 @@ const char *rg_rewrite_head(const uint8_t *m, uint64_t n, const float v[4], std:
 		L.swap(kept);
 	}
 
-	// chain_prepare_for_write_ with use_padding (:1169-1243)
-	uint64_t cur = chain_length(L);
-	const bool tail_pad = L.back().type == 1;
-	if(cur < initial && tail_pad) L.back().length += initial - cur;
-	else if(cur + 4 <= initial) L.push_back(ChainBlock{1, initial - 4 - cur, {}, {}, {}});
-	else if(cur > initial && tail_pad) {
-		const uint64_t delta = cur - initial;
-		if(L.back().length + 4 == delta) L.pop_back();
-		else if(L.back().length >= delta) L.back().length -= delta;
-	}
+	// chain_prepare_for_write_ with use_padding
+	const int64_t pad = chain_padding(initial, chain_length(L), L.back().type == 1 ? (int64_t)L.back().length : -1);
+	if(L.back().type == 1) L.pop_back();
+	if(pad >= 0) L.push_back(ChainBlock{1, (uint64_t)pad, {}, {}, {}});
 	for(ChainBlock &b : L)
 		if(b.length >= (1u << 24)) {
 			if(b.type != 1) return kBlockTooLong;
 			b.length = (1u << 24) - 1;
 		}
-	cur = chain_length(L);
-	*in_place = cur == initial;
+	*in_place = chain_length(L) == initial;
 
-	head->assign(m, m + prefix);
+	head->assign(m, m + r.marker + 4);
 	for(size_t i = 0; i < L.size(); i++) {
 		const ChainBlock &b = L[i];
-		head->push_back((uint8_t)((i + 1 == L.size() ? 0x80 : 0) | b.type));
-		head->push_back((uint8_t)(b.length >> 16));
-		head->push_back((uint8_t)(b.length >> 8));
-		head->push_back((uint8_t)b.length);
+		put_block_header(*head, i + 1 == L.size(), b.type, (uint32_t)b.length);
 		if(b.type == 1) head->insert(head->end(), (size_t)b.length, 0);
 		else head->insert(head->end(), b.body.begin(), b.body.end());
 	}
@@ -220,7 +134,7 @@ const char *rg_rewrite_head(const uint8_t *m, uint64_t n, const float v[4], std:
 namespace {
 
 // The most a file's metadata can grow by: a new VORBIS_COMMENT (header, vendor length, this library's vendor string, entry count)
-// with the five longest entries, "REPLAYGAIN_REFERENCE_LOUDNESS=89.0 dB" (37 bytes), "..._GAIN=-24601.00 dB" (34) and
+// with the five longest entries: the reference loudness "...=89.0 dB" (37 bytes), "..._GAIN=-24601.00 dB" (34) and
 // "..._PEAK=1.00000000" (32) twice. FB200_ADD_REPLAYGAIN_GROWTH is documented as at least this; a vendor string that outgrew it
 // would raise the bound the call checks, never let it write past out_capacity.
 uint64_t growth_bound()

@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "fb200_internal.h"
+#include "flac_metadata.h"
 #include "windows.h"
 
 namespace fb200 {

@@ -275,9 +275,6 @@ struct FlacHeaderPlan {
 	std::vector<uint8_t> blob;
 	std::vector<SeekPt> pts;
 };
-// Checks every file's blocks metadata[metadata_offsets[f] .. [f + 1]) (both may be null: none) and plans the headers;
-// FB200_ERR_INVALID with fb200_last_error naming the file, block and rule.
-int plan_flac_headers(const uint8_t *metadata, const uint64_t *metadata_offsets, uint32_t nfiles, FlacHeaderPlan *plan);
 // k_files_scan + k_files_gather: frames[o] = (frame in encode order, file) of output frame o; writes offsets[0 .. nframes].
 // src holds src_cap bytes of frames (+ 4 readable bytes); frames the encode could not store there are not copied. heads
 // (null: none) leaves each file's header room before its frames, fbase[f] being where the file's first frame goes, and copies
@@ -380,33 +377,6 @@ void launch_pcm_pack(const int32_t *pcm, const FileSeg *segs, const uint32_t *se
 // points build theirs on the device, k_flac_file_headers)
 void put_streaminfo(uint8_t body[34], uint32_t min_blocksize, uint32_t max_blocksize, uint32_t min_framesize, uint32_t max_framesize,
                     uint32_t sample_rate, uint32_t channels, uint32_t bits_per_sample, uint64_t total_samples, const uint8_t md5[16]);
-
-// ---- the metadata lists of fb200_encode_pcm_files_* and fb200_reencode_flac_files_* (pcm_container.cu)
-// One file's blocks after STREAMINFO around its VORBIS_COMMENT: whole blocks (4-byte header and body) before and after it, its
-// entries (the vendor is the encoder's), and a last PADDING block of `padding` bytes (-1: none)
-struct FileMeta {
-	std::vector<uint8_t> before, after;
-	std::vector<std::string> ent;
-	int64_t padding = -1;
-};
-void put_block(std::vector<uint8_t> &m, uint32_t type, const std::vector<uint8_t> &body);
-void put_file_metadata(const FileMeta &M, std::vector<uint8_t> &m);
-// the SEEKTABLE template body of "-S <spacing_s>s" for a file of `samples` (empty: no point)
-std::vector<uint8_t> seek_template(int32_t spacing_s, uint64_t samples, uint32_t sample_rate);
-// flac__utils_set_channel_mask_tag on a VORBIS_COMMENT's entries
-void set_channel_mask_tag(std::vector<std::string> &ent, uint32_t mask);
-// --replay-gain's three tag writes on every file's list (a ReplayGainJob's rebuild, ctx an RgRebuild); without album, the album
-// tags are not written (the tool writes them only when every file of the invocation succeeded)
-struct RgRebuild {
-	std::vector<FileMeta> files;
-	bool album = true;
-};
-int rg_rebuild(void *ctx, const fb200_replaygain_info *info, std::vector<uint8_t> *meta, std::vector<uint64_t> *moffs);
-// FLAC__metadata_object_vorbiscomment_remove_entries_matching: the entries whose field name (before the first '=') is `name`
-// without ASCII case go
-void vorbis_remove_matching(std::vector<std::string> &ent, const char *name);
-// append_tag_ (grabbag/replaygain.c): "name=value" printed with fmt in the C locale
-std::string rg_tag(const char *fmt, const char *name, float value);
 
 // ---- fb200_reencode_flac_files_* (reencode.cu)
 // decoder.cu: the facts a re-encode reads of the batch fb200_decode_files_index left resident (false without one): each file's

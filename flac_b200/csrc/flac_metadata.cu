@@ -2,9 +2,14 @@
 // init_stream_internal_ checks a set_metadata list (stream_encoder.c:869-920) and serialised as FLAC__add_metadata_block writes
 // them (stream_encoder_framing.c:47-243), into one header blob per call. The STREAMINFO body and the SEEKTABLE body are left
 // for k_flac_file_headers, which knows the frame sizes, the MD5 and where each frame landed.
+// It also holds the other host writers of metadata blocks: the lists the batch encoders build for WAV / AIFF and FLAC input, the
+// padding rule of the metadata chain, and the ReplayGain tag edits of flac --replay-gain and metaflac --add-replay-gain.
+#include <locale.h>
 #include <string.h>
+#include <strings.h>
 
-#include "fb200_internal.h"
+#include "flac_metadata.h"
+#include "flac_parse.h"
 
 extern "C" const char *FLAC__VENDOR_STRING;
 
@@ -13,15 +18,6 @@ namespace fb200 {
 namespace {
 
 constexpr unsigned long long kPlaceholder = ~0ull;  // FLAC__STREAM_METADATA_SEEKPOINT_PLACEHOLDER
-
-uint32_t be(const uint8_t *p, int n)
-{
-	uint32_t v = 0;
-	for(int i = 0; i < n; i++) v = (v << 8) | p[i];
-	return v;
-}
-unsigned long long be64(const uint8_t *p) { return ((unsigned long long)be(p, 4) << 32) | be(p + 4, 4); }
-uint32_t le32(const uint8_t *p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 
 // utf8len_ (format.c:322-360) over a bounded string: bytes past the end read as the terminating NUL
 uint32_t utf8len(const uint8_t *s, size_t n, size_t i)
@@ -127,18 +123,7 @@ int plan_flac_headers(const uint8_t *metadata, const uint64_t *metadata_offsets,
 				case 4: {
 					if(has_vc) return bad("a second VORBIS_COMMENT");
 					has_vc = true;
-					uint64_t q = 0;
-					if(len < 8) return bad("VORBIS_COMMENT shorter than its fixed fields");
-					q = 4 + (uint64_t)le32(b);
-					if(q + 4 > len) return bad("VORBIS_COMMENT vendor string runs past the block");
-					const uint32_t nc = le32(b + q);
-					q += 4;
-					for(uint32_t c = 0; c < nc; c++) {
-						if(q + 4 > len) return bad("VORBIS_COMMENT comment runs past the block");
-						q += 4 + (uint64_t)le32(b + q);
-						if(q > len) return bad("VORBIS_COMMENT comment runs past the block");
-					}
-					if(q != len) return bad("VORBIS_COMMENT length differs from its fields");
+					if(const char *why = vorbis_comment_exact(b, len, nullptr)) return bad(why);
 					if(len - le32(b) + vlen >= (1u << 24)) return bad("VORBIS_COMMENT too long with this library's vendor string");
 					break;
 				}
@@ -187,19 +172,12 @@ int plan_flac_headers(const uint8_t *metadata, const uint64_t *metadata_offsets,
 		std::vector<uint8_t> &o = plan->blob;
 		const size_t h0 = o.size();
 		H.blob = h0;
-		auto hdr = [&](bool last, uint32_t type, uint32_t len) {
-			o.push_back((uint8_t)((last ? 0x80 : 0) | type));
-			o.push_back((uint8_t)(len >> 16)); o.push_back((uint8_t)(len >> 8)); o.push_back((uint8_t)len);
-		};
-		auto put_le32 = [&](uint32_t v) { for(int k = 0; k < 4; k++) o.push_back((uint8_t)(v >> (8 * k))); };
 		o.insert(o.end(), {'f', 'L', 'a', 'C'});
-		hdr(false, 0, 34);
+		put_block_header(o, false, 0, 34);
 		o.insert(o.end(), 34, 0);
 		if(!has_vc) {
-			hdr(blks.empty(), 4, 8 + vlen);
-			put_le32(vlen);
-			o.insert(o.end(), FLAC__VENDOR_STRING, FLAC__VENDOR_STRING + vlen);
-			put_le32(0);
+			put_block_header(o, blks.empty(), 4, 8 + vlen);
+			put_vorbis_comment(o, FLAC__VENDOR_STRING, {});
 		}
 		for(size_t i = 0; i < blks.size(); i++) {
 			const Blk &B = blks[i];
@@ -207,11 +185,11 @@ int plan_flac_headers(const uint8_t *metadata, const uint64_t *metadata_offsets,
 			const size_t body = o.size() + 4;
 			switch(B.type) {
 				case 1:  // PADDING: zeros, whatever the caller passed (stream_encoder_framing.c:97-100)
-					hdr(last, 1, B.len);
+					put_block_header(o, last, 1, B.len);
 					o.insert(o.end(), B.len, 0);
 					break;
 				case 3:  // SEEKTABLE: the template's points; the body is written by the device once the frames are placed
-					hdr(last, 3, B.len);
+					put_block_header(o, last, 3, B.len);
 					o.insert(o.end(), B.len, 0);
 					H.st_body = (uint32_t)(body - h0);
 					H.npts = B.len / 18;
@@ -221,32 +199,20 @@ int plan_flac_headers(const uint8_t *metadata, const uint64_t *metadata_offsets,
 					break;
 				case 4: {  // VORBIS_COMMENT: this library's vendor string (stream_encoder_framing.c:66-77, 118-133)
 					const uint32_t old = le32(B.body);
-					hdr(last, 4, B.len - old + vlen);
-					put_le32(vlen);
+					put_block_header(o, last, 4, B.len - old + vlen);
+					put_le32(o, vlen);
 					o.insert(o.end(), FLAC__VENDOR_STRING, FLAC__VENDOR_STRING + vlen);
 					o.insert(o.end(), B.body + 4 + old, B.body + B.len);
 					break;
 				}
 				case 5: {  // CUESHEET: reserved fields as zeros (stream_encoder_framing.c:162-191)
-					hdr(last, 5, B.len);
-					const size_t c0 = o.size();
+					put_block_header(o, last, 5, B.len);
 					o.insert(o.end(), B.body, B.body + B.len);
-					uint8_t *c = o.data() + c0;
-					c[136] &= 0x80;
-					memset(c + 137, 0, 258);
-					size_t p = 396;
-					for(uint32_t t = 0; t < c[395]; t++) {
-						c[p + 21] &= 0xC0;
-						memset(c + p + 22, 0, 13);
-						const uint32_t nidx = c[p + 35];
-						p += 36;
-						for(uint32_t k = 0; k < nidx; k++) memset(c + p + 12 * k + 9, 0, 3);
-						p += 12ull * nidx;
-					}
+					cuesheet_zero_reserved(o.data() + o.size() - B.len, B.len);  // check_cuesheet has passed: the walk is whole
 					break;
 				}
 				default:  // APPLICATION, PICTURE and unknown types: their fields re-serialise to the same bytes
-					hdr(last, B.type, B.len);
+					put_block_header(o, last, B.type, B.len);
 					o.insert(o.end(), B.body, B.body + B.len);
 					break;
 			}
@@ -255,6 +221,170 @@ int plan_flac_headers(const uint8_t *metadata, const uint64_t *metadata_offsets,
 		if(hb >= (1ull << 31)) { set_error("file %u: metadata too large", f); return FB200_ERR_INVALID; }
 		H.bytes = (uint32_t)hb;
 	}
+	return FB200_OK;
+}
+
+void put_block_header(std::vector<uint8_t> &o, bool last, uint32_t type, uint32_t length)
+{
+	o.push_back((uint8_t)((last ? 0x80 : 0) | type));
+	o.push_back((uint8_t)(length >> 16));
+	o.push_back((uint8_t)(length >> 8));
+	o.push_back((uint8_t)length);
+}
+
+void put_vorbis_comment(std::vector<uint8_t> &o, const std::string &vendor, const std::vector<std::string> &ent)
+{
+	put_le32(o, (uint32_t)vendor.size());
+	o.insert(o.end(), vendor.begin(), vendor.end());
+	put_le32(o, (uint32_t)ent.size());
+	for(const std::string &s : ent) {
+		put_le32(o, (uint32_t)s.size());
+		o.insert(o.end(), s.begin(), s.end());
+	}
+}
+
+void put_block(std::vector<uint8_t> &m, uint32_t type, const std::vector<uint8_t> &body)
+{
+	put_block_header(m, false, type, (uint32_t)body.size());
+	m.insert(m.end(), body.begin(), body.end());
+}
+
+std::vector<uint8_t> seek_template(int32_t spacing_s, uint64_t samples, uint32_t sample_rate)
+{
+	std::vector<uint8_t> st;
+	if(spacing_s <= 0 || samples == 0) return st;
+	// grabbag__seektable_convert_specification_to_template "<n>s;" (seektable.c) + append_spaced_points_by_samples
+	// (metadata_object.c:1126-1162)
+	uint32_t spacing = (uint32_t)((double)spacing_s * (double)sample_rate);
+	if(spacing < sample_rate / 2) spacing = sample_rate / 2;
+	if(spacing > 0) {
+		uint64_t num = 1 + samples / spacing;
+		if(samples % spacing == 0) num--;
+		if(num > 32768) {
+			num = 32768;
+			spacing = (uint32_t)(samples / num);
+		}
+		st.assign(18 * num, 0);
+		for(uint64_t j = 0; j < num; j++) {
+			const uint64_t s = j * spacing;
+			for(int b = 0; b < 8; b++) st[18 * j + b] = (uint8_t)(s >> (56 - 8 * b));
+		}
+	}
+	return st;
+}
+
+void set_channel_mask_tag(std::vector<std::string> &ent, uint32_t mask)
+{
+	// flac__utils_set_channel_mask_tag: FLAC__metadata_object_vorbiscomment_replace_comment(all=true) -- the first entry of that
+	// name takes the new value, later ones go; none: appended
+	static const char kName[] = "WAVEFORMATEXTENSIBLE_CHANNEL_MASK";
+	char tag[128];
+	snprintf(tag, sizeof tag, "%s=0x%04X", kName, mask);
+	bool done = false;
+	std::vector<std::string> kept;
+	for(auto &s : ent) {
+		if(!vorbis_entry_matches(s.data(), s.size(), kName)) kept.push_back(s);
+		else if(!done) { kept.push_back(tag); done = true; }
+	}
+	if(!done) kept.push_back(tag);
+	ent.swap(kept);
+}
+
+void put_file_metadata(const FileMeta &M, std::vector<uint8_t> &m)
+{
+	m.insert(m.end(), M.before.begin(), M.before.end());
+	std::vector<uint8_t> vc;
+	put_vorbis_comment(vc, "", M.ent);  // vendor: the encoder writes its own
+	put_block(m, 4, vc);
+	m.insert(m.end(), M.after.begin(), M.after.end());
+	if(M.padding >= 0) put_block(m, 1, std::vector<uint8_t>((size_t)M.padding, 0));
+}
+
+int64_t chain_padding(int64_t initial, int64_t current, int64_t padding)
+{
+	if(current < initial && padding >= 0) return padding + initial - current;  // shrank: the trailing PADDING takes up the room
+	if(current + 4 <= initial) return initial - 4 - current;                    // shrank by a block header or more: a new PADDING
+	if(current > initial && padding >= 0) {                                     // grew: use up or trim the PADDING when it covers the growth
+		const int64_t delta = current - initial;
+		if(padding + 4 == delta) return -1;
+		if(padding >= delta) return padding - delta;
+	}
+	return padding;
+}
+
+// ---- ReplayGain tags (grabbag/replaygain.c:353-500)
+
+const char *const kRgName[5] = {"REPLAYGAIN_REFERENCE_LOUDNESS", "REPLAYGAIN_TRACK_GAIN", "REPLAYGAIN_TRACK_PEAK", "REPLAYGAIN_ALBUM_GAIN",
+                                "REPLAYGAIN_ALBUM_PEAK"};
+
+namespace {
+
+// FLAC__metadata_object_vorbiscomment_remove_entries_matching
+void vorbis_remove_matching(std::vector<std::string> &ent, const char *name)
+{
+	std::vector<std::string> kept;
+	for(auto &s : ent)
+		if(!vorbis_entry_matches(s.data(), s.size(), name)) kept.push_back(s);
+	ent.swap(kept);
+}
+
+// append_tag_: "name=value" printed with fmt in the C locale
+std::string rg_tag(const char *fmt, const char *name, float value)
+{
+	static const locale_t c_locale = newlocale(LC_ALL_MASK, "C", (locale_t)0);
+	const locale_t old = uselocale(c_locale);
+	char buf[256];
+	snprintf(buf, sizeof buf, fmt, name, (double)value);
+	uselocale(old);
+	return buf;
+}
+
+// the bytes --replay-gain's edits can change: the VORBIS_COMMENT block and the PADDING block, headers included (the other blocks
+// keep theirs)
+int64_t edited_length(const FileMeta &M)
+{
+	int64_t n = 4 + 8;
+	for(auto &s : M.ent) n += 4 + (int64_t)s.size();
+	return n + (M.padding >= 0 ? 4 + M.padding : 0);
+}
+
+// One of flac --replay-gain's metadata writes: the edit, then the blocks laid out as the chain write lays them out. The only
+// PADDING block is the last block here, so FLAC__metadata_chain_sort_padding leaves the list as it is. (A FLAC input's list ends
+// in its one PADDING block too, when it has one.)
+void rg_write(FileMeta &M, RgField edit, float gain, float peak)
+{
+	const int64_t initial = edited_length(M);
+	rg_edit(M.ent, edit, gain, peak);
+	M.padding = chain_padding(initial, edited_length(M), M.padding);
+	if(M.padding > (1 << 24) - 1) M.padding = (1 << 24) - 1;
+}
+
+}  // namespace
+
+void rg_edit(std::vector<std::string> &ent, RgField edit, float gain, float peak)
+{
+	static const char *const kFormat[5] = {"%s=%2.1f dB", "%s=%+2.2f dB", "%s=%1.8f", "%s=%+2.2f dB", "%s=%1.8f"};
+	const int n = edit == RG_REFERENCE ? 1 : 2;
+	const float value[2] = {edit == RG_REFERENCE ? 89.0f : gain, peak};
+	for(int i = 0; i < n; i++) vorbis_remove_matching(ent, kRgName[edit + i]);
+	for(int i = 0; i < n; i++) ent.push_back(rg_tag(kFormat[edit + i], kRgName[edit + i], value[i]));
+}
+
+int rg_rebuild(void *ctx, const fb200_replaygain_info *info, std::vector<uint8_t> *meta, std::vector<uint64_t> *moffs)
+{
+	const RgRebuild &R = *static_cast<const RgRebuild *>(ctx);
+	moffs->assign(1, 0);
+	for(size_t f = 0; f < R.files.size(); f++) {
+		FileMeta M = R.files[f];
+		const fb200_replaygain_info &I = info[f];
+		// after each file's encode, the reference and the track tags (main.c:1775-1785); after every file's, the album tags (:575-590)
+		rg_write(M, RG_REFERENCE, 0.f, 0.f);
+		rg_write(M, RG_TRACK_GAIN, I.track_gain, I.track_peak);
+		if(R.album) rg_write(M, RG_ALBUM_GAIN, I.album_gain, I.album_peak);
+		put_file_metadata(M, *meta);
+		moffs->push_back(meta->size());
+	}
+	meta->push_back(0);
 	return FB200_OK;
 }
 

@@ -4,12 +4,11 @@
 // over the whole batch in one launch; the rest is fb200_encode_flac_files_*'s machinery.
 // The other direction (fb200_decode_pcm_files_*, decoder.cu; fb200_pcm_header): the header write_iff_headers writes
 // (decode.c:718-989), built on the host, and k_pcm_pack, which restates write_callback (decode.c:1245-1632) in one launch.
-#include <locale.h>
 #include <stdarg.h>
 #include <string.h>
-#include <strings.h>
 
 #include "fb200_internal.h"
+#include "flac_metadata.h"
 
 namespace fb200 {
 
@@ -598,53 +597,6 @@ void probe_one(const uint8_t *p, uint64_t n, uint64_t base, fb200_pcm_file_info 
 	I->status = FB200_PCM_OK;
 }
 
-}  // namespace
-
-void put_block(std::vector<uint8_t> &m, uint32_t type, const std::vector<uint8_t> &body)
-{
-	m.push_back((uint8_t)type);
-	const uint32_t n = (uint32_t)body.size();
-	m.push_back((uint8_t)(n >> 16));
-	m.push_back((uint8_t)(n >> 8));
-	m.push_back((uint8_t)n);
-	m.insert(m.end(), body.begin(), body.end());
-}
-
-namespace {
-
-void put_le32(std::vector<uint8_t> &v, uint32_t x)
-{
-	for(int i = 0; i < 4; i++) v.push_back((uint8_t)(x >> (8 * i)));
-}
-
-}  // namespace
-
-std::vector<uint8_t> seek_template(int32_t spacing_s, uint64_t samples, uint32_t sample_rate)
-{
-	std::vector<uint8_t> st;
-	if(spacing_s <= 0 || samples == 0) return st;
-	// grabbag__seektable_convert_specification_to_template "<n>s;" (seektable.c) + append_spaced_points_by_samples
-	// (metadata_object.c:1126-1162)
-	uint32_t spacing = (uint32_t)((double)spacing_s * (double)sample_rate);
-	if(spacing < sample_rate / 2) spacing = sample_rate / 2;
-	if(spacing > 0) {
-		uint64_t num = 1 + samples / spacing;
-		if(samples % spacing == 0) num--;
-		if(num > 32768) {
-			num = 32768;
-			spacing = (uint32_t)(samples / num);
-		}
-		st.assign(18 * num, 0);
-		for(uint64_t j = 0; j < num; j++) {
-			const uint64_t s = j * spacing;
-			for(int b = 0; b < 8; b++) st[18 * j + b] = (uint8_t)(s >> (56 - 8 * b));
-		}
-	}
-	return st;
-}
-
-namespace {
-
 // One file's blocks after STREAMINFO, as EncoderSession_init_encoder lists them for a non-FLAC input (encode.c:1945-2020):
 // SEEKTABLE template (when there is one), VORBIS_COMMENT (entries; the vendor is the encoder's), PADDING (padding >= 0)
 void file_metadata(const fb200_pcm_file_info &I, const fb200_pcm_encode_options &opt, const char *tags, size_t tags_len, FileMeta *M)
@@ -665,118 +617,6 @@ void file_metadata(const fb200_pcm_file_info &I, const fb200_pcm_encode_options 
 		M->padding = (int64_t)len;
 	}
 }
-
-}  // namespace
-
-void set_channel_mask_tag(std::vector<std::string> &ent, uint32_t mask)
-{
-	// flac__utils_set_channel_mask_tag: FLAC__metadata_object_vorbiscomment_replace_comment(all=true) -- the first entry of that
-	// name takes the new value, later ones go; none: appended
-	static const char kName[] = "WAVEFORMATEXTENSIBLE_CHANNEL_MASK";
-	char tag[128];
-	snprintf(tag, sizeof tag, "%s=0x%04X", kName, mask);
-	auto named = [&](const std::string &s) { return s.size() > sizeof kName - 1 && s[sizeof kName - 1] == '=' && !strncasecmp(s.c_str(), kName, sizeof kName - 1); };
-	bool done = false;
-	std::vector<std::string> kept;
-	for(auto &s : ent) {
-		if(!named(s)) kept.push_back(s);
-		else if(!done) { kept.push_back(tag); done = true; }
-	}
-	if(!done) kept.push_back(tag);
-	ent.swap(kept);
-}
-
-void put_file_metadata(const FileMeta &M, std::vector<uint8_t> &m)
-{
-	m.insert(m.end(), M.before.begin(), M.before.end());
-	std::vector<uint8_t> vc;
-	put_le32(vc, 0);  // vendor: the encoder writes its own
-	put_le32(vc, (uint32_t)M.ent.size());
-	for(auto &s : M.ent) {
-		put_le32(vc, (uint32_t)s.size());
-		vc.insert(vc.end(), s.begin(), s.end());
-	}
-	put_block(m, 4, vc);
-	m.insert(m.end(), M.after.begin(), M.after.end());
-	if(M.padding >= 0) put_block(m, 1, std::vector<uint8_t>((size_t)M.padding, 0));
-}
-
-namespace {
-
-// ---- --replay-gain's tag edits (grabbag/replaygain.c:353-500, written as store_to_file_post_ writes them)
-
-// the bytes the edits can change: the VORBIS_COMMENT block and the PADDING block, headers included (the other blocks keep theirs)
-int64_t edited_length(const FileMeta &M)
-{
-	int64_t n = 4 + 8;
-	for(auto &s : M.ent) n += 4 + (int64_t)s.size();
-	return n + (M.padding >= 0 ? 4 + M.padding : 0);
-}
-
-// One of the tool's three metadata writes: remove the entries named `names` (FLAC__metadata_object_vorbiscomment_entry_matches:
-// the field name before the first '=' without ASCII case), append `add`, then lay the blocks out as chain_prepare_for_write_
-// with use_padding does (metadata_iterators.c:1169-1224). The only PADDING block is the last block here, so
-// FLAC__metadata_chain_sort_padding leaves the list as it is. (A FLAC input's list ends in its one PADDING block too, when it has one.)
-void rg_write(FileMeta &M, std::initializer_list<const char *> names, std::initializer_list<std::string> add)
-{
-	const int64_t initial = edited_length(M);
-	for(const char *name : names) vorbis_remove_matching(M.ent, name);
-	for(auto &s : add) M.ent.push_back(s);
-	const int64_t cur = edited_length(M);
-	if(cur < initial && M.padding >= 0) M.padding += initial - cur;  // shrank: the last block, PADDING, takes up the room
-	else if(cur + 4 <= initial) M.padding = initial - 4 - cur;        // shrank by a block header or more: a new PADDING
-	else if(cur > initial && M.padding >= 0) {                        // grew: use up or trim the PADDING when it covers the growth
-		const int64_t delta = cur - initial;
-		if(M.padding + 4 == delta) M.padding = -1;
-		else if(M.padding >= delta) M.padding -= delta;
-	}
-	if(M.padding > (1 << 24) - 1) M.padding = (1 << 24) - 1;
-}
-
-}  // namespace
-
-void vorbis_remove_matching(std::vector<std::string> &ent, const char *name)
-{
-	const size_t k = strlen(name);
-	std::vector<std::string> kept;
-	for(auto &s : ent) {
-		const size_t eq = s.find('=');
-		if(!(eq == k && !strncasecmp(s.c_str(), name, k))) kept.push_back(s);
-	}
-	ent.swap(kept);
-}
-
-std::string rg_tag(const char *fmt, const char *name, float value)
-{
-	static const locale_t c_locale = newlocale(LC_ALL_MASK, "C", (locale_t)0);
-	const locale_t old = uselocale(c_locale);
-	char buf[256];
-	snprintf(buf, sizeof buf, fmt, name, (double)value);
-	uselocale(old);
-	return buf;
-}
-
-int rg_rebuild(void *ctx, const fb200_replaygain_info *info, std::vector<uint8_t> *meta, std::vector<uint64_t> *moffs)
-{
-	static const char kRef[] = "REPLAYGAIN_REFERENCE_LOUDNESS", kTG[] = "REPLAYGAIN_TRACK_GAIN", kTP[] = "REPLAYGAIN_TRACK_PEAK",
-	                  kAG[] = "REPLAYGAIN_ALBUM_GAIN", kAP[] = "REPLAYGAIN_ALBUM_PEAK";
-	const RgRebuild &R = *static_cast<const RgRebuild *>(ctx);
-	moffs->assign(1, 0);
-	for(size_t f = 0; f < R.files.size(); f++) {
-		FileMeta M = R.files[f];
-		const fb200_replaygain_info &I = info[f];
-		// after each file's encode, the reference and the track tags (main.c:1775-1785); after every file's, the album tags (:575-590)
-		rg_write(M, {kRef}, {rg_tag("%s=%2.1f dB", kRef, 89.0f)});
-		rg_write(M, {kTG, kTP}, {rg_tag("%s=%+2.2f dB", kTG, I.track_gain), rg_tag("%s=%1.8f", kTP, I.track_peak)});
-		if(R.album) rg_write(M, {kAG, kAP}, {rg_tag("%s=%+2.2f dB", kAG, I.album_gain), rg_tag("%s=%1.8f", kAP, I.album_peak)});
-		put_file_metadata(M, *meta);
-		moffs->push_back(meta->size());
-	}
-	meta->push_back(0);
-	return FB200_OK;
-}
-
-namespace {
 
 int encode_pcm_files(fb200_encoder *e, const uint8_t *data, bool device, const uint64_t *file_offsets, uint32_t nfiles, const fb200_pcm_file_info *info,
                      const fb200_pcm_encode_options *opt, const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *out, size_t out_capacity,

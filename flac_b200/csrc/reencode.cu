@@ -7,20 +7,12 @@
 #include <string.h>
 
 #include "fb200_internal.h"
+#include "flac_metadata.h"
 #include "flac_parse.h"
 
 namespace fb200 {
 
 namespace {
-
-uint32_t le32(const uint8_t *p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
-
-uint64_t be64(const uint8_t *p)
-{
-	uint64_t v = 0;
-	for(int i = 0; i < 8; i++) v = v << 8 | p[i];
-	return v;
-}
 
 // One metadata block as it stands in the file: the 4-byte header (last flag cleared) and the body.
 struct Block {
@@ -34,45 +26,17 @@ struct Block {
 // parsed the same bytes, so this fails only on a region that is not that file's.
 const char *input_blocks(const std::vector<uint8_t> &m, std::vector<Block> *out)
 {
-	size_t pos = 0;
-	if(m.size() >= 10 && memcmp(m.data(), "ID3", 3) == 0) pos = id3v2_tag_bytes(m.data());
-	if(pos > m.size() || m.size() - pos < 4 || memcmp(m.data() + pos, "fLaC", 4) != 0) return "no fLaC marker";
-	pos += 4;
-	for(bool last = false; !last;) {
-		if(m.size() - pos < 4) return "metadata runs past the file";
-		const MetaBlockHeader h = metadata_block_header(m.data() + pos);
-		if(m.size() - pos - 4 < h.length) return "metadata runs past the file";
-		last = h.last;
-		Block b{h.type, std::vector<uint8_t>(m.data() + pos, m.data() + pos + 4 + h.length)};
+	const MetaRegion r = read_metadata_region(m.data(), m.size());
+	if(r.end == MetaRegion::NO_MARKER) return "no fLaC marker";
+	if(r.end == MetaRegion::SHORT) return "metadata runs past the file";
+	for(const MetaBlock &h : r.blocks) {
+		Block b{h.type, std::vector<uint8_t>(m.data() + h.body - 4, m.data() + h.body + h.length)};
 		b.bytes[0] &= 0x7f;
 		out->push_back(std::move(b));
-		pos += 4 + (size_t)h.length;
 	}
 	if(out->empty() || out->front().type != 0) return "first metadata block is not STREAMINFO";  // get_sample_info_flac
 	out->erase(out->begin());
 	return nullptr;
-}
-
-// A VORBIS_COMMENT body's entries; false when its fields disagree with its length
-bool vorbis_entries(const Block &b, std::vector<std::string> *ent)
-{
-	const uint8_t *p = b.body();
-	const size_t n = b.length();
-	size_t pos = 0;
-	if(n < 4 || n - 4 < le32(p)) return false;
-	pos = 4 + (size_t)le32(p);
-	if(n - pos < 4) return false;
-	const uint32_t count = le32(p + pos);
-	pos += 4;
-	for(uint32_t i = 0; i < count; i++) {
-		if(n - pos < 4) return false;
-		const uint32_t l = le32(p + pos);
-		pos += 4;
-		if(n - pos < l) return false;
-		ent->emplace_back(reinterpret_cast<const char *>(p + pos), l);
-		pos += l;
-	}
-	return pos == n;
 }
 
 // encode.c:1782-1795: a CUESHEET with tracks whose lead-out (the last track's offset) is not the input's length is dropped. A
@@ -152,7 +116,7 @@ const char *flac_input_metadata(std::vector<Block> L, const fb200_flac_reencode_
 		if(b.type == 4) {
 			if(at_vc) return "a second VORBIS_COMMENT";
 			at_vc = true;
-			if(!b.bytes.empty() && !vorbis_entries(b, &M->ent)) return "VORBIS_COMMENT fields disagree with the block length";
+			if(!b.bytes.empty() && vorbis_comment_exact(b.body(), b.length(), &M->ent)) return "VORBIS_COMMENT fields disagree with the block length";
 			continue;
 		}
 		std::vector<uint8_t> &to = at_vc ? M->after : M->before;

@@ -6,11 +6,11 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
-#include <strings.h>
 
 #include <mutex>
 
 #include "fb200_internal.h"
+#include "flac_metadata.h"
 #include "flac_parse.h"
 #include "glibc_tanh.cuh"
 
@@ -352,13 +352,10 @@ bool rgs_parse_double(const std::string &entry, double *val)
 }
 
 // FLAC__metadata_object_vorbiscomment_find_entry_from(block, 0, name): the first entry whose name before its first '=' matches
-int rgs_find(const std::vector<std::string> &ent, const char *name)
+int rgs_find(const std::vector<std::string> &ent, RgField field)
 {
-	const size_t k = strlen(name);
-	for(size_t i = 0; i < ent.size(); i++) {
-		const size_t eq = ent[i].find('=');
-		if(eq == k && strncasecmp(ent[i].c_str(), name, k) == 0) return (int)i;
-	}
+	for(size_t i = 0; i < ent.size(); i++)
+		if(vorbis_entry_matches(ent[i].data(), ent[i].size(), kRgName[field])) return (int)i;
 	return -1;
 }
 
@@ -366,11 +363,11 @@ int rgs_find(const std::vector<std::string> &ent, const char *name)
 bool rgs_load(const std::vector<std::string> &ent, bool album, bool strict, double *reference, double *gain, double *peak, bool *album_used)
 {
 	*reference = 89.0;
-	int r = rgs_find(ent, "REPLAYGAIN_REFERENCE_LOUDNESS");
+	int r = rgs_find(ent, RG_REFERENCE);
 	if(r >= 0) (void)rgs_parse_double(ent[r], reference);
 	bool res = true;
-	const int g = rgs_find(ent, album ? "REPLAYGAIN_ALBUM_GAIN" : "REPLAYGAIN_TRACK_GAIN");
-	const int p = rgs_find(ent, album ? "REPLAYGAIN_ALBUM_PEAK" : "REPLAYGAIN_TRACK_PEAK");
+	const int g = rgs_find(ent, album ? RG_ALBUM_GAIN : RG_TRACK_GAIN);
+	const int p = rgs_find(ent, album ? RG_ALBUM_PEAK : RG_TRACK_PEAK);
 	if(g < 0 || p < 0) res = false;
 	if(res && !rgs_parse_double(ent[g], gain)) res = false;
 	if(res && !rgs_parse_double(ent[p], peak)) res = false;
@@ -389,7 +386,7 @@ void rgs_decide(const uint8_t *p, size_t n, uint32_t bps, const fb200_replaygain
 	I->status = FB200_RGS_NO_TAGS;
 	for_each_vorbis_comment(p, n, [&](const uint8_t *b, uint32_t len) {
 		std::vector<std::string> ent;
-		if(!vorbis_entries(b, len, &ent)) return;  // libFLAC fails the block: the callback never sees it
+		if(!read_metadata_vorbiscomment(b, len, &ent)) return;  // libFLAC fails the block: the callback never sees it
 		double reference = 89.0, gain = 0.0, peak = 0.0;
 		bool album_used = false;
 		const bool ok = rgs_load(ent, rg.album != 0, false, &reference, &gain, &peak, &album_used);

@@ -20,6 +20,7 @@
 #include "../../include/flac_b200.h"
 #include "../../include/flac_b200_stream.h"
 #include "fb200_internal.h"
+#include "flac_metadata.h"
 #include "flac_parse.h"
 
 // ------------------------------------------------------------------ small host utilities
@@ -119,7 +120,6 @@ void crc_init()
 struct ByteWriter {
 	std::vector<uint8_t> v;
 	void u(uint64_t val, int nbytes) { for(int i = nbytes - 1; i >= 0; i--) v.push_back((uint8_t)(val >> (8 * i))); }
-	void le32(uint32_t val) { for(int i = 0; i < 4; i++) v.push_back((uint8_t)(val >> (8 * i))); }
 	void raw(const void *p, size_t n) { const uint8_t *b = (const uint8_t *)p; v.insert(v.end(), b, b + n); }
 	void zeros(size_t n) { v.insert(v.end(), n, 0); }
 };
@@ -153,10 +153,10 @@ bool serialize_metadata(const FLAC__StreamMetadata *m, bool is_last, const char 
 		case FLAC__METADATA_TYPE_VORBIS_COMMENT: {
 			// the encoder always writes its own vendor string (stream_encoder_framing.c:118-133)
 			const uint32_t vlen = (uint32_t)strlen(vendor);
-			body.le32(vlen); body.raw(vendor, vlen);
-			body.le32(m->data.vorbis_comment.num_comments);
+			fb200::put_le32(body.v, vlen); body.raw(vendor, vlen);
+			fb200::put_le32(body.v, m->data.vorbis_comment.num_comments);
 			for(uint32_t i = 0; i < m->data.vorbis_comment.num_comments; i++) {
-				body.le32(m->data.vorbis_comment.comments[i].length);
+				fb200::put_le32(body.v, m->data.vorbis_comment.comments[i].length);
 				body.raw(m->data.vorbis_comment.comments[i].entry, m->data.vorbis_comment.comments[i].length);
 			}
 			break;
@@ -191,10 +191,8 @@ bool serialize_metadata(const FLAC__StreamMetadata *m, bool is_last, const char 
 			break;
 	}
 	if(body.v.size() >= (1u << 24)) return false;
-	ByteWriter hdr;
-	hdr.u((is_last ? 0x80 : 0) | ((uint32_t)m->type & 0x7f), 1);
-	hdr.u(body.v.size(), 3);
-	out = hdr.v;
+	out.clear();
+	fb200::put_block_header(out, is_last, (uint32_t)m->type & 0x7f, (uint32_t)body.v.size());
 	out.insert(out.end(), body.v.begin(), body.v.end());
 	return true;
 }
@@ -1035,15 +1033,13 @@ static bool dec_read_metadata(FLAC__StreamDecoder *d)
 			pts.resize(len / 18);
 			for(size_t i = 0; i < pts.size(); i++) {
 				const uint8_t *s = b + 18 * i;
-				uint64_t sn = 0, so = 0;
-				for(int k = 0; k < 8; k++) { sn = (sn << 8) | s[k]; so = (so << 8) | s[8 + k]; }
-				pts[i].sample_number = sn; pts[i].stream_offset = so; pts[i].frame_samples = (s[16] << 8) | s[17];
+				pts[i].sample_number = fb200::be64(s); pts[i].stream_offset = fb200::be64(s + 8); pts[i].frame_samples = fb200::be(s + 16, 2);
 			}
 			m.data.seek_table.num_points = (uint32_t)pts.size(); m.data.seek_table.points = pts.data();
 		}
 		else if(type == FLAC__METADATA_TYPE_VORBIS_COMMENT && len >= 8) {
 			size_t pos = 0;
-			auto rd = [&](uint32_t &v) { if(pos + 4 > len) return false; v = b[pos] | (b[pos + 1] << 8) | (b[pos + 2] << 16) | ((uint32_t)b[pos + 3] << 24); pos += 4; return true; };
+			auto rd = [&](uint32_t &v) { if(pos + 4 > len) return false; v = fb200::le32(b + pos); pos += 4; return true; };
 			uint32_t vl = 0, nc = 0;
 			bool ok = rd(vl) && pos + vl <= len;
 			if(ok) { strs.emplace_back(b + pos, b + pos + vl); strs.back().push_back(0); pos += vl; ok = rd(nc); }

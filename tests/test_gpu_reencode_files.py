@@ -279,6 +279,15 @@ def test_replay_gain_album(rate):
         assert o == w
 
 
+def vorbis_comment_block(entries, count=None, tail=b""):
+    """a VORBIS_COMMENT whose entry count (default: the entries') and trailing bytes may disagree with its entries"""
+    le = lambda v: v.to_bytes(4, "little")
+    body = le(5) + b"other" + le(len(entries) if count is None else count)
+    for e in entries:
+        body += le(len(e)) + e
+    return fb.metadata_block(fb.METADATA_VORBIS_COMMENT, body + tail)
+
+
 def damaged_inputs():
     good = [make_flac(30000 + 1000 * k, 2, 16, 44100, seed=70 + k) for k in range(2)]
     base = make_flac(30000, 2, 16, 44100, seed=80)
@@ -294,9 +303,13 @@ def damaged_inputs():
     bad_md5[8 + 18] ^= 1
     seek = fb.seektable_block([(44100, 0, 0), (0, 0, 0)])
     bad_seek = with_blocks(base, [seek])
+    # the tool's decoder fails a VORBIS_COMMENT with bytes after its last entry; the encoder takes one VORBIS_COMMENT at most
+    vc_bytes_left = with_blocks(base, [vorbis_comment_block([b"A=1"], tail=b"\0\0"), fb.padding_block(10)])
+    two_vcs = with_blocks(base, [vorbis_comment_block([b"A=1"]), fb.padding_block(10), vorbis_comment_block([b"B=2"])])
     assert bytes(si) == bytes(base[8:42])
     return good, [(bytes(no_total), fb.REENCODE_NO_TOTAL), (bytes(flipped), fb.REENCODE_DAMAGED), (bytes(truncated), fb.REENCODE_DAMAGED),
-                  (bytes(bad_md5), fb.REENCODE_MD5_MISMATCH), (bad_seek, fb.REENCODE_METADATA)]
+                  (bytes(bad_md5), fb.REENCODE_MD5_MISMATCH), (bad_seek, fb.REENCODE_METADATA), (vc_bytes_left, fb.REENCODE_METADATA),
+                  (two_vcs, fb.REENCODE_METADATA)]
 
 
 def test_failures():
@@ -311,6 +324,25 @@ def test_failures():
         assert out[1] == b"" and info[1].file.bytes == 0
         for k in (0, 2):
             assert out[k] == tool(blobs[k], tool_args(5))[1]
+
+
+@pytest.mark.parametrize("tags", [
+    pytest.param(None, id="input_tags", marks=pytest.mark.xfail(strict=True, reason=(
+        "the tool's decoder keeps the entries that fit (read_metadata_vorbiscomment_) and re-encodes the file; the input list "
+        "reads the block with the encoder's rule that its fields fill it exactly, and fails the file"))),
+    pytest.param(["TITLE=x"], id="new_tags"),
+])
+def test_vorbis_comment_count_past_block(tags):
+    """A VORBIS_COMMENT whose count claims more entries than the block holds: the tool re-encodes the file; with -T, the
+    input's VORBIS_COMMENT goes unread."""
+    need_tool()
+    base = make_flac(30000, 2, 16, 44100, seed=81)
+    blob = with_blocks(base, [vorbis_comment_block([b"A=1", b"B=2"], count=3), fb.padding_block(10)])
+    rc, want = tool(blob, tool_args(5, tags=tags))
+    assert rc == 0
+    out, info = ours([blob], 5, tags=tags)
+    assert info[0].status == fb.REENCODE_OK, info[0].error
+    assert out[0] == want
 
 
 def reencode_raw(enc, dec, files, replay_gain=False, reserved=0, tags=None, tag_offsets=None):
