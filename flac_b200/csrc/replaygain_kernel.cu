@@ -215,13 +215,17 @@ __global__ void __launch_bounds__(32) k_replaygain_frames(const int32_t *__restr
 	uint32_t pk = 0;
 	bool ok = states[F.state].errors == 0;
 	unsigned long long next = F.audio;  // where the next accepted frame must begin
+	unsigned long long next_sample = ~0ull;  // where the next frame's samples must begin (none before the first frame)
 	for(unsigned long long i = F.cand0; ok && i < F.cand0 + F.ncand; i++) {
 		const FilePlace p = place[i];
 		if(p.n == 0) continue;
 		const FileDecCand cd = cands[i];
 		const uint32_t bs = cd.blocksize;
-		if(begins[i] != next || cd.rate_differs || p.n != bs * ch) { ok = false; break; }
+		// a gap in the sample numbers is a missing frame: libFLAC reports MISSING_FRAME (stream_decoder.c:2487-2494) and
+		// metaflac fails the file, even when the frames around it tile the bytes
+		if(begins[i] != next || cd.rate_differs || p.n != bs * ch || (next_sample != ~0ull && cd.first_sample > next_sample)) { ok = false; break; }
 		next = begins[i] + bytes[i];
+		next_sample = cd.first_sample + bs;
 		const int32_t *fr = pcm + p.dst + cc;
 		for(uint32_t s0 = 0; s0 < bs; s0 += kRgCall) {
 			const uint32_t len = min(kRgCall, bs - s0), m = len / ds;

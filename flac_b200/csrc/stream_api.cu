@@ -900,6 +900,9 @@ struct FLAC__StreamDecoderPrivate {
 	std::vector<int32_t> residual;                        // scratch: residuals of the frame being delivered (FLAC__Subframe.residual)
 	uint64_t expect_pos;          // byte offset (in `audio`) where the next frame should start
 	bool lost_sync_reported;
+	FLAC__FrameHeader last_header;  // the header of the last frame written, silence included (stream_decoder.c:3580-3581)
+	bool last_set;
+	bool error_sent;              // an error was reported while finding the frame now being delivered (error_has_been_sent)
 	std::vector<int32_t> planar;
 	MD5 md5;
 	uint64_t samples_decoded;
@@ -1132,8 +1135,56 @@ static bool dec_decode_batch(FLAC__StreamDecoder *d, size_t first)
 	return true;
 }
 
+static void dec_error(FLAC__StreamDecoder *d, FLAC__StreamDecoderErrorStatus status)
+{
+	FLAC__StreamDecoderPrivate *q = d->private_;
+	q->error_sent = true;
+	if(q->error_cb) q->error_cb(d, status, q->client_data);
+}
+
+// A gap in the sample numbers before the frame `next` (stream_decoder.c:2483-2554): MISSING_FRAME unless an error was already
+// reported while finding `next`; then, when the last written frame agrees with `next` on rate, channels and bits per sample and
+// has at least 16 samples, silence frames shaped like it (its header, the sample number advanced by its blocksize, the last one
+// shortened), at most 5 seconds and 50 of its blocks. Past those caps the gap stays: the stream comes out shorter.
+static bool dec_fill_gap(FLAC__StreamDecoder *d, const FrameIndexEntry &next, uint64_t next_sample)
+{
+	FLAC__StreamDecoderPrivate *q = d->private_;
+	if(!q->last_set) return true;
+	const FLAC__FrameHeader &last = q->last_header;
+	if(last.number.sample_number + last.blocksize >= next_sample) return true;
+	uint32_t need = (uint32_t)(next_sample - (last.number.sample_number + last.blocksize));  // uint32_t as in the reference
+	if(!q->error_sent) dec_error(d, FLAC__STREAM_DECODER_ERROR_STATUS_MISSING_FRAME);
+	if(last.sample_rate != next.sample_rate || last.channels != next.channels || last.bits_per_sample != next.bps || last.blocksize < 16)
+		return true;
+	need = std::min(need, 5 * last.sample_rate);
+	need = std::min(need, 50 * last.blocksize);
+	FLAC__Frame fr;
+	memset(&fr, 0, sizeof fr);
+	fr.header = last;
+	for(uint32_t c = 0; c < last.channels; c++) fr.subframes[c].type = FLAC__SUBFRAME_TYPE_CONSTANT;
+	std::vector<int32_t> zero((size_t)last.blocksize * last.channels, 0);
+	const int32_t *chan[FLAC__MAX_CHANNELS];
+	for(uint32_t c = 0; c < last.channels; c++) chan[c] = zero.data();
+	while(need) {
+		fr.header.number.sample_number += fr.header.blocksize;
+		if(need < fr.header.blocksize) fr.header.blocksize = need;
+		need -= fr.header.blocksize;
+		d->protected_->blocksize = fr.header.blocksize;
+		q->samples_decoded = fr.header.number.sample_number + fr.header.blocksize;
+		if(d->protected_->md5_checking && !q->did_seek)
+			q->md5.update_samples(zero.data(), (size_t)fr.header.blocksize * fr.header.channels, (fr.header.bits_per_sample + 7) / 8);
+		q->last_header = fr.header;
+		if(q->write_cb(d, &fr, chan, q->client_data) != FLAC__STREAM_DECODER_WRITE_STATUS_CONTINUE) {
+			d->protected_->state = FLAC__STREAM_DECODER_ABORTED;
+			return false;
+		}
+	}
+	return true;
+}
+
 // hand one frame to the client (write_audio_frame_to_client_, stream_decoder.c:3578-3635); frames that fail are reported
-// through the error callback and NOT delivered, like the reference (stream_decoder.c:2443-2590)
+// through the error callback and NOT delivered, like the reference (stream_decoder.c:2443-2590), and a gap they leave in the
+// sample numbers is filled with the reference's silence frames
 static bool dec_deliver_next(FLAC__StreamDecoder *d)
 {
 	FLAC__StreamDecoderPrivate *q = d->private_;
@@ -1145,20 +1196,20 @@ static bool dec_deliver_next(FLAC__StreamDecoder *d)
 		const FrameIndexEntry &fe = q->index[q->next_frame];
 		const uint32_t st = q->batch_status[bi] & 0xffu;
 		if(fe.offset < q->expect_pos && !q->did_seek) { q->next_frame++; continue; }  // a header look-alike inside the previous frame
+		q->error_sent = false;  // the reference clears error_has_been_sent after every frame it reads, good or bad (:2556)
 		if(st != 0) {
 			// a broken frame (or a look-alike in junk): report once per damaged stretch, move on to the next candidate
-			if(q->error_cb) {
-				const FLAC__StreamDecoderErrorStatus es = st == 7 ? FLAC__STREAM_DECODER_ERROR_STATUS_FRAME_CRC_MISMATCH :
-				    (st == 2 || st == 3) ? FLAC__STREAM_DECODER_ERROR_STATUS_BAD_HEADER :
-				    st == 4 ? FLAC__STREAM_DECODER_ERROR_STATUS_UNPARSEABLE_STREAM : FLAC__STREAM_DECODER_ERROR_STATUS_LOST_SYNC;
-				q->error_cb(d, es, q->client_data);
-			}
+			dec_error(d, st == 7 ? FLAC__STREAM_DECODER_ERROR_STATUS_FRAME_CRC_MISMATCH :
+			             (st == 2 || st == 3) ? FLAC__STREAM_DECODER_ERROR_STATUS_BAD_HEADER :
+			             st == 4 ? FLAC__STREAM_DECODER_ERROR_STATUS_UNPARSEABLE_STREAM :
+			             st == 9 ? FLAC__STREAM_DECODER_ERROR_STATUS_OUT_OF_BOUNDS : FLAC__STREAM_DECODER_ERROR_STATUS_LOST_SYNC);
 			q->next_frame++;
 			continue;
 		}
-		if(fe.offset > q->expect_pos && !q->did_seek && q->expect_pos != 0 && q->error_cb)
-			q->error_cb(d, FLAC__STREAM_DECODER_ERROR_STATUS_LOST_SYNC, q->client_data);  // junk between two frames
+		if(fe.offset > q->expect_pos && !q->did_seek && q->expect_pos != 0)
+			dec_error(d, FLAC__STREAM_DECODER_ERROR_STATUS_LOST_SYNC);  // junk between two frames
 		q->expect_pos = fe.offset + q->batch_bytes[bi];
+		if(!dec_fill_gap(d, fe, q->first_sample[q->next_frame])) return false;
 		break;
 	}
 	const size_t bi = q->next_frame - q->batch_first;
@@ -1221,6 +1272,7 @@ static bool dec_deliver_next(FLAC__StreamDecoder *d)
 	if(d->protected_->md5_checking && !q->did_seek) q->md5.update_samples(src, (size_t)bs * ch, (fe.bps + 7) / 8);
 	q->samples_decoded = first_sample + bs;
 	d->protected_->state = FLAC__STREAM_DECODER_SEARCH_FOR_FRAME_SYNC;
+	q->last_header = fr.header; q->last_set = true;
 	if(q->write_cb(d, &fr, chan, q->client_data) != FLAC__STREAM_DECODER_WRITE_STATUS_CONTINUE) {
 		d->protected_->state = FLAC__STREAM_DECODER_ABORTED;
 		return false;
@@ -1307,7 +1359,7 @@ static FLAC__StreamDecoderInitStatus dec_init_common(FLAC__StreamDecoder *d)
 {
 	FLAC__StreamDecoderPrivate *q = d->private_;
 	q->in.clear(); q->in_pos = 0; q->consumed_before_in = 0; q->audio_offset = 0; q->eof = false; q->metadata_done = false; q->indexed = false; q->has_streaminfo = false; q->did_seek = false;
-	q->next_frame = 0; q->skip_samples = 0; q->batch_first = q->batch_count = 0; q->samples_decoded = 0;
+	q->next_frame = 0; q->skip_samples = 0; q->batch_first = q->batch_count = 0; q->samples_decoded = 0; q->last_set = false; q->error_sent = false;
 	memset(&q->si, 0, sizeof q->si);
 	d->protected_->state = FLAC__STREAM_DECODER_SEARCH_FOR_METADATA;
 	return FLAC__STREAM_DECODER_INIT_STATUS_OK;
@@ -1390,7 +1442,7 @@ FLAC__bool FLAC__stream_decoder_reset(FLAC__StreamDecoder *d)
 {
 	if(DEC_UNINIT(d)) return false;
 	FLAC__StreamDecoderPrivate *q = d->private_;
-	if(q->indexed) { q->next_frame = 0; q->skip_samples = 0; q->batch_count = 0; q->did_seek = false; q->expect_pos = 0; q->md5.init(); d->protected_->state = FLAC__STREAM_DECODER_SEARCH_FOR_FRAME_SYNC; return true; }
+	if(q->indexed) { q->next_frame = 0; q->skip_samples = 0; q->batch_count = 0; q->did_seek = false; q->expect_pos = 0; q->last_set = false; q->md5.init(); d->protected_->state = FLAC__STREAM_DECODER_SEARCH_FOR_FRAME_SYNC; return true; }
 	return !q->metadata_done && q->in.empty();
 }
 
@@ -1466,6 +1518,7 @@ FLAC__bool FLAC__stream_decoder_seek_absolute(FLAC__StreamDecoder *d, FLAC__uint
 	q->next_frame = lo;
 	q->skip_samples = sample - q->first_sample[lo];
 	q->did_seek = true;
+	q->last_set = false;  // the frame a seek lands on is not compared with what came before it (is_seeking, :2484)
 	d->protected_->state = FLAC__STREAM_DECODER_SEARCH_FOR_FRAME_SYNC;
 	return dec_deliver_next(d);  // the reference delivers the frame containing the target right away (stream_decoder.c:1282-1340)
 }

@@ -438,7 +438,7 @@ int fb200_debug_replaygain_windows(int device, const int32_t *d_pcm, uint64_t pc
  *  1. Pre-checks: a file the index did not pass is INPUT; a file whose rate, bits or channels differ from the album's first file's,
  *     or whose rate the filters do not cover, or that has 3 or more channels, is FORMAT. Either fails the album.
  *  2. Analysis: every file is decoded with MD5 checking off. Any decode error fails the album with DECODE: a damaged or missing
- *     frame, a frame whose header codes a sample rate other than STREAMINFO's, and any byte of the audio region that no accepted
+ *     frame (a gap in the sample numbers between two frames included, where libFLAC reports MISSING_FRAME), a frame whose header codes a sample rate other than STREAMINFO's, and any byte of the audio region that no accepted
  *     frame covers (the frames must tile [audio_offset_in, end of file) exactly: junk between or after the frames, a truncated last
  *     frame). The analysis feeds the filters frame by frame in calls of at most 2048 samples, as grabbag__replaygain_analyze does
  *     (each call decimates from its own start and drops its remainder; after a call of m < 10 decimated samples the filter's input
@@ -663,8 +663,23 @@ int fb200_decode_indexed_host(fb200_decoder *dec, const uint64_t *begins, uint32
  * Output: the files back to back in file order, each interleaved with its own channel count and `samples` long (STREAMINFO's
  * total_samples; when that is 0, the end of the file's last frame header found). Frames are cut at `samples`; samples that no
  * accepted frame covers are zero. A lost frame in the middle of a file is therefore silence, as the reference delivers it
- * (stream_decoder.c:2483-2554); a lost first or last frame keeps the file's length, where the reference delivers a shorter
- * stream. With do_md5, each decoded file's MD5 (its samples as (bps + 7) / 8-byte little-endian integers, md5.c:280-521) is
+ * (stream_decoder.c:2483-2554), with one difference: the reference writes at most 50 of the previous frame's blocks or 5
+ * seconds of silence, whichever is less, and then the next frame early, while here every frame stays at its sample number, so
+ * a longer gap is all zeros and the file keeps its length. A lost first or last frame keeps the file's length, where the
+ * reference delivers a shorter stream. Other known differences from libFLAC on damaged files:
+ *  - header_disagrees: a frame whose channels, bits per sample or blocksize disagree with STREAMINFO is not indexed, so its
+ *    samples are lost; libFLAC decodes and writes it.
+ *  - overlap: a frame that starts before the end of the frame placed before it (a repeated or reordered frame) is not
+ *    placed, its samples are zeros unless another frame covers them, and it counts as an error; libFLAC writes every frame in
+ *    stream order.
+ *  - lost_without_candidate: `errors` counts damaged stretches the index found a candidate in; a frame lost with its header
+ *    (a damaged header, or frames cut out) shows only in samples_missing, where libFLAC reports lost sync, a bad header or a
+ *    missing frame.
+ *  - trailing_junk: the drop-in decoder reports nothing for bytes after the last frame (an ID3v1 or APE tag); libFLAC
+ *    reports them as lost sync.
+ *  - junk: junk that carries no frame header (and ID3v1 / APE tags) is never seen by the index; libFLAC reports it as lost
+ *    sync.
+ * With do_md5, each decoded file's MD5 (its samples as (bps + 7) / 8-byte little-endian integers, md5.c:280-521) is
  * computed on the device and compared with STREAMINFO's; an all-zero STREAMINFO MD5 is not checked.
  *
  * Candidates are decoded into a scratch of at most FB200_DECODE_FILES_SAMPLE_BUDGET samples (all channels, int32) per launch
@@ -726,6 +741,9 @@ int fb200_decode_files_device(fb200_decoder *dec, int32_t *d_pcm, uint64_t pcm_c
  * candidate; an accepted frame overlapping the previous placed one is not placed; the part of each placed frame inside the
  * range is copied, and samples no accepted frame covers are zero (samples_missing). So a range's output equals the same slice
  * of fb200_decode_files_* output whenever no false header candidate passes CRC-16, and a lost frame inside a range is silence.
+ * Known divergence (range_sees_its_frames): a range walks only the frames that meet it, so a frame the whole-file decode drops
+ * because an earlier frame in the file ends past its first sample (swapped or moved frames) is placed by a range that does not
+ * meet that earlier frame.
  * No MD5 is computed (the reference turns MD5 checking off after a seek). The resident index is not changed: decode_files_*
  * afterwards returns what it returned before; the next index call replaces the batch for both. The per-frame status of
  * fb200_decoder_get_frame_status is left untouched. */
