@@ -313,6 +313,19 @@ def lib():
                                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p]
     L.fb200_reencode_flac_files_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(FlacReencodeOptions), C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p]
+    L.fb200_encode_pcm_files_ranges_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(PcmEncodeOptions),
+                                                     C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                     C.POINTER(C.c_uint64), C.c_void_p]
+    L.fb200_encode_pcm_files_ranges_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(PcmEncodeOptions),
+                                                       C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                       C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p]
+    L.fb200_reencode_flac_files_ranges_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(FlacReencodeOptions),
+                                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p]
+    L.fb200_reencode_flac_files_ranges_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(FlacReencodeOptions),
+                                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_uint64),
+                                                          C.c_void_p, C.c_void_p]
+    L.fb200_skip_until.restype = C.c_int
+    L.fb200_skip_until.argtypes = [C.c_char_p, C.c_char_p, C.c_uint32, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     L.fb200_encoder_set_verify.argtypes = [C.c_void_p, C.c_int]
     L.fb200_replaygain_device.restype = C.c_int
     L.fb200_replaygain_device.argtypes = [C.c_int, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
@@ -493,6 +506,16 @@ def probe_pcm_files(blobs, data=None, offsets=None):
     arr = (PcmFileInfo * max(n, 1))()
     _check(lib().fb200_pcm_files_probe(data.ctypes.data, int(offsets[-1]), offsets.ctypes.data, n, arr))
     return list(arr[:n])
+
+
+def skip_until(skip, until, rate, total):
+    """flac --skip=skip --until=until (str each, None = not given) for a stream of `total` samples per channel at `rate` Hz:
+    (first_sample, samples) as the tool computes them. Raises FlacB200Error (code -3, the tool's message) where the tool
+    refuses the pair, and for a range of 0 samples."""
+    first, n = C.c_uint64(0), C.c_uint64(0)
+    enc = lambda v: None if v is None else str(v).encode()
+    _check(lib().fb200_skip_until(enc(skip), enc(until), rate, total, C.byref(first), C.byref(n)))
+    return first.value, n.value
 
 
 def _tags(tags, nfiles):
@@ -880,82 +903,106 @@ class Encoder:
                                                     d_out_ptr, out_capacity, d_offsets_ptr, C.byref(nf), arr, C.c_void_p(stream)))
         return nf.value, list(arr[:lengths.size])
 
-    def pcm_files_capacity(self, infos, tags=None, padding=-1, replay_gain=False):
-        """Output bytes that always suffice for encode_pcm_files* of these probed files."""
-        lengths = [int(i.samples) for i in infos]
+    def pcm_files_capacity(self, infos, tags=None, padding=-1, replay_gain=False, ranges=None):
+        """Output bytes that always suffice for encode_pcm_files* of these probed files (or of these (file, first_sample,
+        samples) ranges of them)."""
+        if ranges is not None:  # a range naming no file makes the call fail: it needs no room
+            q = [(int(f), int(n)) for f, _, n in np.asarray(ranges, dtype=np.uint64).reshape(-1, 3) if f < len(infos)]
+            infos = [infos[f] for f, _ in q]
+            lengths = declared = [n for _, n in q]
+        else:
+            lengths, declared = [int(i.samples) for i in infos], [int(i.declared) for i in infos]
         _, cap = self.files_capacity(lengths)
         tb, _ = _tags(tags, len(infos))
         extra = 0
-        for i in infos:
-            points = min(32768, int(i.declared) // max(i.sample_rate // 2, 1) + 1)
+        for i, d in zip(infos, declared):
+            points = min(32768, d // max(i.sample_rate // 2, 1) + 1)
             extra += 18 * points + (0 if not padding else padding if padding > 0 else 65536) + 42 + 8 + 64 + 256 + 64 + (190 if replay_gain else 0)
         return cap + extra + (0 if tb is None else tb.size + 4 * tb.size)
 
-    def _pcm_call(self, host, data, offsets, infos, tags, seek_spacing_s, padding, md5, out, out_capacity, frame_offsets, stream=0, replay_gain=False):
+    def _pcm_call(self, host, data, offsets, infos, tags, seek_spacing_s, padding, md5, out, out_capacity, frame_offsets, stream=0, replay_gain=False,
+                  ranges=None):
         n = len(infos)
         arr = (PcmFileInfo * max(n, 1))(*infos)
-        files = (FlacFileInfo * max(n, 1))()
-        tb, toffs = _tags(tags, n)
+        if ranges is not None:
+            rarr, nout = Decoder.sample_ranges(ranges)
+        else:
+            nout = n
+        files = (FlacFileInfo * max(nout, 1))()
+        tb, toffs = _tags(tags, nout)
         opt = PcmEncodeOptions(seek_spacing_s, padding, 1 if md5 else 0, 1 if replay_gain else 0)
         nf = C.c_uint64(0)
-        args = [self._h, data, offsets.ctypes.data, n, arr, C.byref(opt), None if tb is None else tb.ctypes.data,
-                None if toffs is None else toffs.ctypes.data, out, out_capacity, frame_offsets, C.byref(nf), files]
-        if host:
-            _check(lib().fb200_encode_pcm_files_host(*args))
+        head = [self._h, data, offsets.ctypes.data, n, arr, C.byref(opt)]
+        tail = [None if tb is None else tb.ctypes.data, None if toffs is None else toffs.ctypes.data, out, out_capacity, frame_offsets, C.byref(nf), files]
+        if ranges is not None:
+            if host:
+                _check(lib().fb200_encode_pcm_files_ranges_host(*head, rarr, nout, *tail))
+            else:
+                _check(lib().fb200_encode_pcm_files_ranges_device(*head, rarr, nout, *tail, C.c_void_p(stream)))
+        elif host:
+            _check(lib().fb200_encode_pcm_files_host(*head, *tail))
         else:
-            _check(lib().fb200_encode_pcm_files_device(*args, C.c_void_p(stream)))
-        return nf.value, list(files[:n])
+            _check(lib().fb200_encode_pcm_files_device(*head, *tail, C.c_void_p(stream)))
+        return nf.value, list(files[:nout])
 
-    def encode_pcm_files(self, blobs, tags=None, seek_spacing_s=10, padding=-1, md5=True, infos=False, replay_gain=False):
+    def encode_pcm_files(self, blobs, tags=None, seek_spacing_s=10, padding=-1, md5=True, infos=False, replay_gain=False, ranges=None):
         """flac [-T ...] [-S <n>s] [-P n] [--replay-gain] *.wav in one call: every file (bytes of a WAV / RF64 / Wave64 / AIFF /
         AIFF-C file) must probe OK with this encoder's channels, bits per sample and rate. tags: None, one list of "NAME=value"
         for every file, or one list per file. seek_spacing_s 0 = -S-, padding -1 = the tool's default, 0 = --no-padding.
-        replay_gain: the REPLAYGAIN_* tags, the call's files being one album. Returns one bytes per file (with infos=True,
+        replay_gain: the REPLAYGAIN_* tags, the call's files being one album. ranges: None, or (file, first_sample, samples) per
+        output ((n, 3) array or list): one .flac per range, as flac --skip=first_sample --until=first_sample+samples writes it
+        (tags then per range; only the files a range names must probe OK). Returns one bytes per file or range (with infos=True,
         ([bytes], [FlacFileInfo]))."""
         data, offsets = _batch(blobs)
         pinfo = probe_pcm_files(None, data, offsets)
-        out = np.empty(self.pcm_files_capacity(pinfo, tags, padding, replay_gain), dtype=np.uint8)
+        out = np.empty(self.pcm_files_capacity(pinfo, tags, padding, replay_gain, ranges), dtype=np.uint8)
         _, files = self._pcm_call(True, data.ctypes.data, offsets, pinfo, tags, seek_spacing_s, padding, md5, out.ctypes.data, out.size, None,
-                                  replay_gain=replay_gain)
+                                  replay_gain=replay_gain, ranges=ranges)
         res = [out[int(i.offset):int(i.offset + i.bytes)].tobytes() for i in files]
         return (res, files) if infos else res
 
     def encode_pcm_files_device(self, d_data_ptr, offsets, pinfo, d_out_ptr, out_capacity, d_offsets_ptr=None, tags=None, seek_spacing_s=10,
-                                padding=-1, md5=True, stream=0, replay_gain=False):
+                                padding=-1, md5=True, stream=0, replay_gain=False, ranges=None):
         """Device-resident encode_pcm_files: the files back to back at d_data_ptr (offsets[n + 1] into it, host), probed as
         probe_pcm_files(None, host copy, offsets) found them; out and (optional) frame offsets are device pointers. Returns
-        (nframes, [FlacFileInfo per file])."""
+        (nframes, [FlacFileInfo per file, or per range with ranges])."""
         offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
         return self._pcm_call(False, d_data_ptr, offsets, pinfo, tags, seek_spacing_s, padding, md5, d_out_ptr, out_capacity, d_offsets_ptr, stream,
-                              replay_gain)
+                              replay_gain, ranges)
 
-    def reencode_capacity(self, decoder, files, tags=None, seek_spacing_s=-1, padding=-1, replay_gain=False):
-        """Output bytes that always suffice for reencode_flac_files* of these files of the decoder's indexed batch."""
+    def reencode_capacity(self, decoder, files, tags=None, seek_spacing_s=-1, padding=-1, replay_gain=False, lengths=None):
+        """Output bytes that always suffice for reencode_flac_files* of these files of the decoder's indexed batch (lengths:
+        samples encoded per entry when not the files' totals, as for ranges)."""
         infos, sizes = decoder._files_infos, decoder._files_sizes
-        lengths = [max(int(infos[f].total_samples), 1) for f in files]
+        if lengths is None:
+            lengths = [max(int(infos[f].total_samples), 1) for f in files]
         _, cap = self.files_capacity(lengths)
         tb, _ = _tags(tags, len(files))
         extra = 0
-        for f in files:
+        for f, n in zip(files, lengths):
             i = infos[f]
-            points = min(32768, int(i.total_samples) // max(i.sample_rate // 2, 1) + 1)
+            points = min(32768, int(n) // max(i.sample_rate // 2, 1) + 1)
             # the input's metadata (at most its file), a new seek table, VORBIS_COMMENT and PADDING
             extra += sizes[f] + 18 * points + max(padding, 65536) + 42 + 8 + 64 + 256 + 64 + (190 if replay_gain else 0)
         return cap + extra + (0 if tb is None else tb.size + 4 * tb.size)
 
-    def _reencode_call(self, host, decoder, files, tags, seek_spacing_s, padding, replay_gain, out, out_capacity, frame_offsets, stream=0):
-        files = np.ascontiguousarray(files, dtype=np.uint32)
-        n = files.size
+    def _reencode_call(self, host, decoder, files, tags, seek_spacing_s, padding, replay_gain, out, out_capacity, frame_offsets, stream=0, ranges=None):
+        if ranges is not None:
+            arg, n = Decoder.sample_ranges(ranges)
+        else:
+            files = np.ascontiguousarray(files, dtype=np.uint32)
+            arg, n = files.ctypes.data, files.size
         info = (FlacReencodeInfo * max(n, 1))()
         tb, toffs = _tags(tags, n)
         opt = FlacReencodeOptions(seek_spacing_s, padding, 1 if replay_gain else 0, 0)
         nf = C.c_uint64(0)
-        args = [self._h, decoder._h, files.ctypes.data, n, C.byref(opt), None if tb is None else tb.ctypes.data, None if toffs is None else toffs.ctypes.data,
+        args = [self._h, decoder._h, arg, n, C.byref(opt), None if tb is None else tb.ctypes.data, None if toffs is None else toffs.ctypes.data,
                 out, out_capacity, frame_offsets, C.byref(nf), info]
-        if host:
-            _check(lib().fb200_reencode_flac_files_host(*args))
+        if ranges is not None:
+            fn = lib().fb200_reencode_flac_files_ranges_host if host else lib().fb200_reencode_flac_files_ranges_device
         else:
-            _check(lib().fb200_reencode_flac_files_device(*args, C.c_void_p(stream)))
+            fn = lib().fb200_reencode_flac_files_host if host else lib().fb200_reencode_flac_files_device
+        _check(fn(*args) if host else fn(*args, C.c_void_p(stream)))
         return nf.value, list(info[:n])
 
     def reencode_flac_files(self, decoder, files, tags=None, seek_spacing_s=-1, padding=-1, replay_gain=False, infos=False):
@@ -975,6 +1022,26 @@ class Encoder:
         """Device-resident reencode_flac_files: out and (optional) frame offsets are device pointers. Returns (nframes,
         [FlacReencodeInfo per file]); file f is out[info.file.offset, + info.file.bytes) when its status is REENCODE_OK."""
         return self._reencode_call(False, decoder, files, tags, seek_spacing_s, padding, replay_gain, d_out_ptr, out_capacity, d_offsets_ptr, stream)
+
+    def reencode_ranges_capacity(self, decoder, ranges, tags=None, seek_spacing_s=-1, padding=-1, replay_gain=False):
+        """Output bytes that always suffice for reencode_flac_ranges* of these (file, first_sample, samples) ranges."""
+        q = [(int(f), int(n)) for f, _, n in np.asarray(ranges, dtype=np.uint64).reshape(-1, 3) if f < len(decoder._files_infos)]
+        return self.reencode_capacity(decoder, [f for f, _ in q], tags, seek_spacing_s, padding, replay_gain, [n for _, n in q])
+
+    def reencode_flac_ranges(self, decoder, ranges, tags=None, seek_spacing_s=-1, padding=-1, replay_gain=False, infos=False):
+        """flac -f --skip --until [-T ...] [-S ..] [-P n] [--replay-gain] *.flac in one call: one .flac per (file, first_sample,
+        samples) range ((n, 3) array or list) of the batch decoder.index_files left resident, as the tool writes it for
+        --skip=first_sample --until=first_sample+samples; options and results as reencode_flac_files, tags per range."""
+        out = np.empty(self.reencode_ranges_capacity(decoder, ranges, tags, seek_spacing_s, padding, replay_gain), dtype=np.uint8)
+        _, info = self._reencode_call(True, decoder, None, tags, seek_spacing_s, padding, replay_gain, out.ctypes.data, out.size, None, ranges=ranges)
+        res = [out[int(i.file.offset):int(i.file.offset + i.file.bytes)].tobytes() for i in info]
+        return (res, info) if infos else res
+
+    def reencode_flac_ranges_device(self, decoder, ranges, d_out_ptr, out_capacity, d_offsets_ptr=None, tags=None, seek_spacing_s=-1, padding=-1,
+                                    replay_gain=False, stream=0):
+        """Device-resident reencode_flac_ranges. Returns (nframes, [FlacReencodeInfo per range])."""
+        return self._reencode_call(False, decoder, None, tags, seek_spacing_s, padding, replay_gain, d_out_ptr, out_capacity, d_offsets_ptr, stream,
+                                   ranges=ranges)
 
     def set_verify(self, on=True):
         """flac -V for encode_files / encode_files_device: every frame is decoded on the device and compared with the input; a

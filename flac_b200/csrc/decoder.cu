@@ -917,10 +917,12 @@ static int ranges_layout(const fb200_decoder *d, const fb200_sample_range *range
 // Decodes the ranges whose layout ranges_layout() gave into d_out (int32, total values, zeroed first). Returns after completion
 // with nframes / samples_missing / candidates of info[] filled (and errors[r], when given, with range r's damaged stretches +
 // overlapping frames). The resident index is only read. With kept, the place of every candidate selected for range r is copied to
-// (*kept)[kept0[r] ..], info[r].candidates of them.
+// (*kept)[kept0[r] ..], info[r].candidates of them. With d_segs (nsegs of them, a batch's FileSeg pairs), info[r].first_value is
+// a value index in the back-to-back numbering of FileSeg::src and the frames are placed through the segments into d_out, the
+// compacted layout `total` values long (decoder_decode_into's placement).
 static int decode_files_ranges_impl(fb200_decoder *d, const fb200_sample_range *ranges, uint32_t nranges, int32_t *d_out, uint64_t total,
                                     fb200_range_decode_info *info, cudaStream_t st, uint32_t *errors = nullptr, std::vector<FilePlace> *kept = nullptr,
-                                    std::vector<uint64_t> *kept0 = nullptr)
+                                    std::vector<uint64_t> *kept0 = nullptr, const FileSeg *d_segs = nullptr, int nsegs = 0)
 {
 	const uint32_t nfiles = (uint32_t)d->files_info.size(), ngroups = (uint32_t)d->files_groups.size();
 	const FilesIndexLayout L(d->files_ncand, d->files_state0.size());
@@ -1033,7 +1035,7 @@ static int decode_files_ranges_impl(fb200_decoder *d, const fb200_sample_range *
 		const FilesRun R{&d->files_groups[g], c0, c1 - c0, states.data() + a, d_states + a, b - a, d_rbeg, d_rend, d_rcands};
 		if(kept) rc = decode_files_run(d, R, d_stat, reinterpret_cast<uint32_t *>(d->d_keep + k_bytes), reinterpret_cast<FilePlace *>(d->d_keep), d_out, st,
 		                               nullptr, 0, true);
-		else rc = decode_files_run(d, R, d_stat, d_bytes, d_place, d_out, st);
+		else rc = decode_files_run(d, R, d_stat, d_bytes, d_place, d_out, st, d_segs, nsegs);
 		if(rc != FB200_OK) return rc;
 	}
 	if(kept) {
@@ -1465,6 +1467,25 @@ int decoder_decode_into(fb200_decoder *d, const uint32_t *files, const uint64_t 
 		if((rc = decode_files_run(d, R, d_stat, keep ? keep_bytes : d_bytes, keep ? keep_place : d_place, pcm, st, d_segs, nsegs, keep)) != FB200_OK) return rc;
 	}
 	FB_CUDA(cudaGetLastError());
+	return FB200_OK;
+}
+
+int decoder_decode_ranges_into(fb200_decoder *d, const fb200_sample_range *ranges, const uint64_t *first_value, uint32_t n, int32_t *pcm,
+                               unsigned long long values, const FileSeg *d_segs, int nsegs, cudaStream_t st, uint32_t *errors, uint64_t *missing)
+{
+	std::vector<fb200_range_decode_info> info(n);
+	for(uint32_t i = 0; i < n; i++) {
+		const fb200_file_decode_info &I = d->files_info[ranges[i].file];
+		memset(&info[i], 0, sizeof info[i]);
+		info[i].status = FB200_FILE_OK;
+		info[i].channels = I.channels;
+		info[i].bits_per_sample = I.bits_per_sample;
+		info[i].first_value = first_value[i];
+		info[i].values = ranges[i].samples * I.channels;
+	}
+	const int rc = decode_files_ranges_impl(d, ranges, n, pcm, values, info.data(), st, errors, nullptr, nullptr, d_segs, nsegs);
+	if(rc != FB200_OK) return rc;
+	for(uint32_t i = 0; i < n; i++) missing[i] = info[i].samples_missing;
 	return FB200_OK;
 }
 

@@ -393,6 +393,12 @@ uint32_t decoder_file_mask(const fb200_decoder *d, uint32_t f);
 // frame byte count stay (a listed file's accepted frames are its candidates with place n > 0, in file order).
 int decoder_decode_into(fb200_decoder *d, const uint32_t *files, const uint64_t *first_value, uint32_t n, int32_t *pcm, unsigned long long values,
                         const FileSeg *d_segs, int nsegs, cudaStream_t st, FilePlace *keep_place = nullptr, uint32_t *keep_bytes = nullptr);
+// decoder.cu: the ranged decode (fb200_decode_files_ranges_*) of ranges[0 .. n) of the resident batch, each over a file whose index
+// status is OK and within its samples, range i's samples to the back-to-back value first_value[i] on, placed through d_segs into pcm
+// (zeroed first, `values` long). Returns after completion with each range's damaged stretches + overlapping frames (errors) and
+// samples no accepted frame covered (missing).
+int decoder_decode_ranges_into(fb200_decoder *d, const fb200_sample_range *ranges, const uint64_t *first_value, uint32_t n, int32_t *pcm,
+                               unsigned long long values, const FileSeg *d_segs, int nsegs, cudaStream_t st, uint32_t *errors, uint64_t *missing);
 // per listed file, after decoder_decode_into and a synchronise: damaged stretches and samples no accepted frame covered
 int decoder_decode_verdicts(fb200_decoder *d, const uint32_t *files, uint32_t n, cudaStream_t st, uint32_t *errors, uint64_t *missing);
 // ---- fb200_add_replaygain_flac_files_* (add_replaygain.cu): the resident index on the device, and one file's place in it: bytes

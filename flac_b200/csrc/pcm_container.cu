@@ -598,10 +598,11 @@ void probe_one(const uint8_t *p, uint64_t n, uint64_t base, fb200_pcm_file_info 
 }
 
 // One file's blocks after STREAMINFO, as EncoderSession_init_encoder lists them for a non-FLAC input (encode.c:1945-2020):
-// SEEKTABLE template (when there is one), VORBIS_COMMENT (entries; the vendor is the encoder's), PADDING (padding >= 0)
-void file_metadata(const fb200_pcm_file_info &I, const fb200_pcm_encode_options &opt, const char *tags, size_t tags_len, FileMeta *M)
+// SEEKTABLE template (when there is one), VORBIS_COMMENT (entries; the vendor is the encoder's), PADDING (padding >= 0). length is
+// total_samples_to_encode: the declared count, or the --skip / --until range's length (encode.c:2010, 2226)
+void file_metadata(const fb200_pcm_file_info &I, uint64_t length, const fb200_pcm_encode_options &opt, const char *tags, size_t tags_len, FileMeta *M)
 {
-	const std::vector<uint8_t> st = seek_template(opt.seek_spacing_s, I.declared, I.sample_rate);
+	const std::vector<uint8_t> st = seek_template(opt.seek_spacing_s, length, I.sample_rate);
 	if(!st.empty()) put_block(M->before, 3, st);
 	std::vector<std::string> &ent = M->ent;
 	for(size_t p = 0; p < tags_len;) {
@@ -612,19 +613,32 @@ void file_metadata(const fb200_pcm_file_info &I, const fb200_pcm_encode_options 
 	if(I.channel_mask) set_channel_mask_tag(ent, I.channel_mask);
 	if(opt.padding != 0) {
 		// with --replay-gain, room for its tags (GRABBAG__REPLAYGAIN_MAX_TAG_SPACE_REQUIRED, encode.c:2004-2011)
-		uint64_t len = (opt.padding > 0 ? (uint64_t)opt.padding : (I.declared / I.sample_rate < 20 * 60 ? 8192 : 65536)) + (opt.replay_gain ? 190 : 0);
+		uint64_t len = (opt.padding > 0 ? (uint64_t)opt.padding : (length / I.sample_rate < 20 * 60 ? 8192 : 65536)) + (opt.replay_gain ? 190 : 0);
 		if(len > (1u << 24) - 1) len = (1u << 24) - 1;
 		M->padding = (int64_t)len;
 	}
 }
 
+// ranges == nullptr: every file whole (flac *.wav); else one output per range (flac --skip=first --until=first+samples)
 int encode_pcm_files(fb200_encoder *e, const uint8_t *data, bool device, const uint64_t *file_offsets, uint32_t nfiles, const fb200_pcm_file_info *info,
-                     const fb200_pcm_encode_options *opt, const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *out, size_t out_capacity,
-                     uint64_t *frame_offsets, uint64_t *nframes, fb200_flac_file_info *files, void *cuda_stream)
+                     const fb200_pcm_encode_options *opt, const fb200_sample_range *ranges, uint32_t nranges, const uint8_t *tags,
+                     const uint64_t *tag_offsets, uint8_t *out, size_t out_capacity, uint64_t *frame_offsets, uint64_t *nframes,
+                     fb200_flac_file_info *files, void *cuda_stream)
 {
 	if(!e || !data || !file_offsets || !info || !opt || !files) { set_error("a required pointer is NULL"); return FB200_ERR_INVALID; }
 	if(nfiles == 0) { set_error("no files"); return FB200_ERR_INVALID; }
 	if(!tags != !tag_offsets) { set_error("tags and tag_offsets must both be given or both be NULL"); return FB200_ERR_INVALID; }
+	if(ranges && (nranges == 0 || nranges >= 0x80000000u)) { set_error("invalid number of ranges %u", nranges); return FB200_ERR_INVALID; }
+	const uint32_t nout = ranges ? nranges : nfiles;
+	const char *unit = ranges ? "range" : "file";
+	std::vector<uint8_t> used(nfiles, ranges ? 0 : 1);
+	for(uint32_t r = 0; ranges && r < nranges; r++) {
+		const fb200_sample_range &q = ranges[r];
+		if(q.file >= nfiles) { set_error("range %u: file %u of a batch of %u", r, q.file, nfiles); return FB200_ERR_INVALID; }
+		if(q.samples == 0) { set_error("range %u is empty", r); return FB200_ERR_INVALID; }
+		if(q.first_sample + q.samples < q.first_sample) { set_error("range %u: first_sample + samples overflows", r); return FB200_ERR_INVALID; }
+		used[q.file] = 1;
+	}
 	fb200_encoder_config cfg;
 	fb200_encoder_get_config(e, &cfg);
 	const uint64_t begin = file_offsets[0], end = file_offsets[nfiles];
@@ -632,17 +646,17 @@ int encode_pcm_files(fb200_encoder *e, const uint8_t *data, bool device, const u
 	PcmSource src;
 	src.data = data + begin;
 	src.bytes = end - begin;
-	src.files.resize(nfiles);
-	std::vector<uint64_t> samples(nfiles), moffs(nfiles + 1, 0);
+	src.files.resize(nout);
+	std::vector<uint64_t> samples(nout), moffs(nout + 1, 0);
 	std::vector<uint8_t> meta;
 	RgRebuild rgr;
-	rgr.files.resize(opt->replay_gain ? nfiles : 0);
+	rgr.files.resize(opt->replay_gain ? nout : 0);
 	ReplayGainJob rg{0, 0, 0, {}, rg_rebuild, &rgr};
 	if(opt->replay_gain) src.rg = &rg;
-	uint64_t elem = 0;
 	for(uint32_t f = 0; f < nfiles; f++) {
 		const fb200_pcm_file_info &I = info[f];
 		if(file_offsets[f + 1] < file_offsets[f]) { set_error("file_offsets decrease at file %u", f); return FB200_ERR_INVALID; }
+		if(!used[f]) continue;
 		if(I.status != FB200_PCM_OK) { set_error("file %u was not probed OK: %s", f, I.error); return FB200_ERR_INVALID; }
 		if(I.channels != cfg.channels || I.bits_per_sample != cfg.bits_per_sample || I.sample_rate != cfg.sample_rate) {
 			set_error("file %u is %u ch / %u bits / %u Hz, the encoder %u / %u / %u", f, I.channels, I.bits_per_sample, I.sample_rate, cfg.channels,
@@ -661,25 +675,38 @@ int encode_pcm_files(fb200_encoder *e, const uint8_t *data, bool device, const u
 			set_error("info of file %u does not describe this batch's file %u", f, f);
 			return FB200_ERR_INVALID;
 		}
-		if(tags && (tag_offsets[f + 1] < tag_offsets[f] || (tag_offsets[f + 1] > tag_offsets[f] && tags[tag_offsets[f + 1] - 1] != 0))) {
-			set_error("tags of file %u do not end in a NUL", f);
+	}
+	uint64_t elem = 0;
+	for(uint32_t r = 0; r < nout; r++) {
+		const uint32_t f = ranges ? ranges[r].file : r;
+		const fb200_pcm_file_info &I = info[f];
+		// the tool's checks after canonicalising --skip / --until against the declared count (encode.c:1043, 2296); a range past the
+		// samples present is refused here, where the tool writes an empty stream
+		const uint64_t first = ranges ? ranges[r].first_sample : 0, length = ranges ? ranges[r].samples : I.declared;
+		if(first > I.declared) { set_error("range %u of file %u: value of --skip exceeds input size", r, f); return FB200_ERR_INVALID; }
+		if(first + length > I.declared) { set_error("range %u of file %u: --until value is after end of input", r, f); return FB200_ERR_INVALID; }
+		if(first >= I.samples) { set_error("range %u of file %u starts at sample %llu, past the %llu samples present", r, f, (unsigned long long)first, (unsigned long long)I.samples); return FB200_ERR_INVALID; }
+		if(tags && (tag_offsets[r + 1] < tag_offsets[r] || (tag_offsets[r + 1] > tag_offsets[r] && tags[tag_offsets[r + 1] - 1] != 0))) {
+			set_error("tags of %s %u do not end in a NUL", unit, r);
 			return FB200_ERR_INVALID;
 		}
-		src.files[f] = PcmFileDev{elem, I.data_offset - begin, B, I.is_big_endian ? 1u : 0u, I.is_unsigned ? 1u : 0u, I.shift};
-		samples[f] = I.samples;
-		elem += I.samples * I.channels;
+		const uint32_t B = I.container_bits / 8;
+		const uint64_t present = (first + length < I.samples ? first + length : I.samples) - first;
+		src.files[r] = PcmFileDev{elem, I.data_offset - begin + first * I.channels * B, B, I.is_big_endian ? 1u : 0u, I.is_unsigned ? 1u : 0u, I.shift};
+		samples[r] = present;
+		elem += present * I.channels;
 		FileMeta M;
-		file_metadata(I, *opt, tags ? reinterpret_cast<const char *>(tags) + tag_offsets[f] : nullptr, tags ? tag_offsets[f + 1] - tag_offsets[f] : 0, &M);
+		file_metadata(I, length, *opt, tags ? reinterpret_cast<const char *>(tags) + tag_offsets[r] : nullptr, tags ? tag_offsets[r + 1] - tag_offsets[r] : 0, &M);
 		put_file_metadata(M, meta);
-		moffs[f + 1] = meta.size();
+		moffs[r + 1] = meta.size();
 		if(opt->replay_gain) {
 			// EncoderSession_process analyses the values format_input shifted down, scaled by the container's bits
 			rg.bps.push_back(I.container_bits);
-			rgr.files[f] = std::move(M);
+			rgr.files[r] = std::move(M);
 		}
 	}
 	meta.push_back(0);
-	return encode_pcm_files_impl(e, src, device, samples.data(), nfiles, opt->md5 ? 1 : 0, meta.data(), moffs.data(), out, out_capacity, frame_offsets, nframes,
+	return encode_pcm_files_impl(e, src, device, samples.data(), nout, opt->md5 ? 1 : 0, meta.data(), moffs.data(), out, out_capacity, frame_offsets, nframes,
 	                             files, cuda_stream);
 }
 
@@ -702,15 +729,145 @@ int fb200_encode_pcm_files_host(fb200_encoder *e, const uint8_t *data, const uin
                                 const fb200_pcm_encode_options *opt, const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *out, size_t out_capacity,
                                 uint64_t *frame_offsets, uint64_t *nframes, fb200_flac_file_info *files)
 {
-	return encode_pcm_files(e, data, false, file_offsets, nfiles, info, opt, tags, tag_offsets, out, out_capacity, frame_offsets, nframes, files, nullptr);
+	return encode_pcm_files(e, data, false, file_offsets, nfiles, info, opt, nullptr, 0, tags, tag_offsets, out, out_capacity, frame_offsets, nframes, files,
+	                        nullptr);
 }
 
 int fb200_encode_pcm_files_device(fb200_encoder *e, const uint8_t *d_data, const uint64_t *file_offsets, uint32_t nfiles, const fb200_pcm_file_info *info,
                                   const fb200_pcm_encode_options *opt, const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *d_out, size_t out_capacity,
                                   uint64_t *d_frame_offsets, uint64_t *nframes, fb200_flac_file_info *files, void *cuda_stream)
 {
-	return encode_pcm_files(e, d_data, true, file_offsets, nfiles, info, opt, tags, tag_offsets, d_out, out_capacity, d_frame_offsets, nframes, files,
-	                        cuda_stream);
+	return encode_pcm_files(e, d_data, true, file_offsets, nfiles, info, opt, nullptr, 0, tags, tag_offsets, d_out, out_capacity, d_frame_offsets, nframes,
+	                        files, cuda_stream);
+}
+
+int fb200_encode_pcm_files_ranges_host(fb200_encoder *e, const uint8_t *data, const uint64_t *file_offsets, uint32_t nfiles, const fb200_pcm_file_info *info,
+                                       const fb200_pcm_encode_options *opt, const fb200_sample_range *ranges, uint32_t nranges, const uint8_t *tags,
+                                       const uint64_t *tag_offsets, uint8_t *out, size_t out_capacity, uint64_t *frame_offsets, uint64_t *nframes,
+                                       fb200_flac_file_info *files)
+{
+	if(!ranges) { set_error("ranges is NULL"); return FB200_ERR_INVALID; }
+	return encode_pcm_files(e, data, false, file_offsets, nfiles, info, opt, ranges, nranges, tags, tag_offsets, out, out_capacity, frame_offsets, nframes,
+	                        files, nullptr);
+}
+
+int fb200_encode_pcm_files_ranges_device(fb200_encoder *e, const uint8_t *d_data, const uint64_t *file_offsets, uint32_t nfiles,
+                                         const fb200_pcm_file_info *info, const fb200_pcm_encode_options *opt, const fb200_sample_range *ranges,
+                                         uint32_t nranges, const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *d_out, size_t out_capacity,
+                                         uint64_t *d_frame_offsets, uint64_t *nframes, fb200_flac_file_info *files, void *cuda_stream)
+{
+	if(!ranges) { set_error("ranges is NULL"); return FB200_ERR_INVALID; }
+	return encode_pcm_files(e, d_data, true, file_offsets, nfiles, info, opt, ranges, nranges, tags, tag_offsets, d_out, out_capacity, d_frame_offsets,
+	                        nframes, files, cuda_stream);
+}
+
+// ---- flac [--skip] [--until]: the tool's arithmetic (utils.c:50-107, 326-398; main.c:1659-1670; encode.c:1003-1081, 2257-2303)
+
+namespace {
+
+// local__parse_uint64_
+bool parse_u64(const char *s, uint64_t *v)
+{
+	uint64_t r = 0;
+	if(!*s) return false;
+	for(char c; (c = *s++) != '\0';) {
+		if(c < '0' || c > '9') return false;
+		if(r > UINT64_MAX / 10) return false;
+		const uint64_t t = r * 10 + (uint64_t)(c - '0');
+		if(r == UINT64_MAX / 10 && t < r) return false;
+		r = t;
+	}
+	*v = r;
+	return true;
+}
+
+// local__parse_timecode_: [0-9]+:[0-9.,]* read by strtod in the C locale
+bool parse_timecode(const char *s, double *v)
+{
+	char c = *s++;
+	if(c < '0' || c > '9') return false;
+	uint32_t i = (uint32_t)(c - '0');
+	while((c = *s++) != ':') {
+		if(c < '0' || c > '9') return false;
+		i = i * 10 + (uint32_t)(c - '0');
+	}
+	if(strspn(s, "1234567890.,") != strlen(s)) return false;
+	char *end;
+	const double d = strtod(s, &end);
+	if(end == s || *end) return false;
+	*v = (double)i * 60. + d;
+	return true;
+}
+
+struct SkipUntil {
+	bool relative = false, is_samples = true;
+	int64_t samples = 0;
+	double seconds = 0;
+};
+
+// flac__utils_parse_skip_until_specification
+bool parse_spec(const char *s, SkipUntil *o)
+{
+	*o = SkipUntil{};
+	if(!s) return true;
+	bool neg = false;
+	if(s[0] == '-') { neg = o->relative = true; s++; }
+	else if(s[0] == '+') { o->relative = true; s++; }
+	uint64_t v;
+	if(parse_u64(s, &v)) {
+		if(v > (uint64_t)INT64_MAX) return false;
+		o->samples = neg ? -(int64_t)v : (int64_t)v;
+		return true;
+	}
+	double d;
+	if(!parse_timecode(s, &d)) return false;
+	o->is_samples = false;
+	o->seconds = neg ? -d : d;
+	return true;
+}
+
+// flac__utils_canonicalize_skip_until_specification: seconds to samples, truncated
+bool canonicalize(SkipUntil *o, uint32_t rate)
+{
+	if(o->is_samples) return true;
+	const double x = o->seconds * (double)rate;
+	if(x >= (double)INT64_MAX || x <= (double)INT64_MIN) return false;
+	o->samples = (int64_t)x;
+	o->is_samples = true;
+	return true;
+}
+
+}  // namespace
+
+int fb200_skip_until(const char *skip, const char *until, uint32_t sample_rate, uint64_t total_samples, uint64_t *first_sample, uint64_t *samples)
+{
+	if(!first_sample || !samples) { set_error("a required pointer is NULL"); return FB200_ERR_INVALID; }
+	*first_sample = *samples = 0;
+	SkipUntil S, U;
+	if(!parse_spec(skip, &S) || S.relative) { set_error("invalid value for --skip"); return FB200_ERR_INVALID; }
+	if(!parse_spec(until, &U)) { set_error("invalid value for --until"); return FB200_ERR_INVALID; }
+	if(!until) U.relative = true;  // no --until is --until=-0
+	if(!canonicalize(&S, sample_rate)) { set_error("value of --skip is too large"); return FB200_ERR_INVALID; }
+	const uint64_t s = (uint64_t)S.samples;
+	// canonicalize_until_specification; 0 means end of stream
+	uint64_t u = 0;
+	if(!canonicalize(&U, sample_rate)) { set_error("value of --until is too large"); return FB200_ERR_INVALID; }
+	if(!(U.relative && U.samples == 0)) {
+		if(total_samples == 0) { set_error("cannot use --until when input length is unknown"); return FB200_ERR_INVALID; }
+		int64_t v = U.samples;
+		if(U.relative) v = (int64_t)((uint64_t)v + (U.samples <= 0 ? total_samples : s));  // two's complement, as the tool's int64 sum
+		if(v < 0) { set_error("--until value is before beginning of input"); return FB200_ERR_INVALID; }
+		if((uint64_t)v <= s) { set_error("--until value is before --skip point"); return FB200_ERR_INVALID; }
+		if((uint64_t)v > total_samples) { set_error("--until value is after end of input"); return FB200_ERR_INVALID; }
+		u = (uint64_t)v;
+	}
+	if(s > total_samples) { set_error("value of --skip exceeds input size"); return FB200_ERR_INVALID; }
+	const uint64_t n = (u ? u : total_samples) - s;
+	// the tool writes a stream without frames here; this engine encodes no empty file
+	if(n == 0) { set_error("--skip leaves no samples to encode"); return FB200_ERR_INVALID; }
+	*first_sample = s;
+	*samples = n;
+	return FB200_OK;
 }
 
 int fb200_pcm_header(const fb200_pcm_decode_options *opt, uint32_t channels, uint32_t bits_per_sample, uint32_t sample_rate, uint32_t channel_mask,

@@ -60,8 +60,10 @@ bool cuesheet_lead_out_wrong(const Block &b, uint64_t total)
 
 // EncoderSession_init_encoder's list for a FLAC input (encode.c:1710-1939) into M; nullptr or why the list cannot be written
 // around a single VORBIS_COMMENT (a second one, or one whose fields disagree with its length: the encoder rejects both).
+// length is total_samples_to_encode (the input's total_samples, or the --skip / --until range's length); whole says it equals
+// the input's total_samples, the one case an input SEEKTABLE can be kept in.
 const char *flac_input_metadata(std::vector<Block> L, const fb200_flac_reencode_options &opt, const std::vector<std::string> &tags, uint32_t mask_tag,
-                                uint64_t total, uint32_t rate, FileMeta *M)
+                                uint64_t length, bool whole, uint32_t rate, FileMeta *M)
 {
 	const Block kNewVc{4, {}}, kNewSt{3, {}};  // markers: the VORBIS_COMMENT and SEEKTABLE this policy makes
 	// VORBIS_COMMENT (:1730-1770): with tags, the input's go and their channel mask tag carries over
@@ -78,17 +80,19 @@ const char *flac_input_metadata(std::vector<Block> L, const fb200_flac_reencode_
 		M->ent = tags;
 		if(!tags.empty() && mask_tag) set_channel_mask_tag(M->ent, mask_tag);
 	}
-	// CUESHEET (:1772-1822)
+	// CUESHEET (:1772-1822): the lead-out is compared with the length encoded; track offsets are not moved
 	{
 		std::vector<Block> kept;
 		for(Block &b : L)
-			if(!(b.type == 5 && cuesheet_lead_out_wrong(b, total))) kept.push_back(std::move(b));
+			if(!(b.type == 5 && cuesheet_lead_out_wrong(b, length))) kept.push_back(std::move(b));
 		L.swap(kept);
 	}
-	// SEEKTABLE (:1824-1880): the input's goes with any -S; a template goes first with -S <n>s, or when there is none
+	// SEEKTABLE (:1824-1880): the input's goes with any -S or when the length changes; a template goes first with -S <n>s, or when
+	// none is left
 	bool st_found = false;
 	for(const Block &b : L) st_found |= b.type == 3 && !b.bytes.empty();
-	if(opt.seek_spacing_s >= 0) {
+	if(opt.seek_spacing_s >= 0 || !whole) {
+		st_found = false;
 		std::vector<Block> kept;
 		for(Block &b : L)
 			if(!(b.type == 3 && !b.bytes.empty())) kept.push_back(std::move(b));
@@ -106,7 +110,7 @@ const char *flac_input_metadata(std::vector<Block> L, const fb200_flac_reencode_
 		L.swap(kept);
 	}
 	if(opt.padding > 0) p = opt.padding;
-	if(p < 0) p = total / rate < 20 * 60 ? 8192 : 65536;
+	if(p < 0) p = length / rate < 20 * 60 ? 8192 : 65536;
 	if(p > 0 && opt.replay_gain) p += 190;  // GRABBAG__REPLAYGAIN_MAX_TAG_SPACE_REQUIRED
 	if(p > (1 << 24) - 1) p = (1 << 24) - 1;
 	M->padding = opt.padding != 0 && p > 0 ? p : -1;
@@ -120,7 +124,7 @@ const char *flac_input_metadata(std::vector<Block> L, const fb200_flac_reencode_
 			continue;
 		}
 		std::vector<uint8_t> &to = at_vc ? M->after : M->before;
-		if(b.type == 3 && b.bytes.empty()) put_block(to, 3, seek_template(opt.seek_spacing_s > 0 ? opt.seek_spacing_s : 10, total, rate));
+		if(b.type == 3 && b.bytes.empty()) put_block(to, 3, seek_template(opt.seek_spacing_s > 0 ? opt.seek_spacing_s : 10, length, rate));
 		else to.insert(to.end(), b.bytes.begin(), b.bytes.end());
 	}
 	return nullptr;
@@ -136,6 +140,8 @@ void fail(fb200_flac_reencode_info &I, uint32_t status, const char *fmt, ...)
 }
 
 // What the encode's hooks share: the files it encodes (batch index, back-to-back first value, STREAMINFO MD5) and their verdicts.
+// With ranges (fb200_reencode_flac_files_ranges_*), what is encoded is range[i] of file batch[i]: the ranged decode fills it and
+// leaves its verdicts in errors / missing, and no input MD5 is compared (the tool zeroes it with --skip or --until, encode.c:1130).
 struct Reencode {
 	fb200_decoder *dec;
 	std::vector<uint32_t> batch;
@@ -143,12 +149,20 @@ struct Reencode {
 	std::vector<uint32_t> status;  // FB200_REENCODE_* after check()
 	RgRebuild *rg = nullptr;
 	bool all_ok = true;            // every listed file passed the host plan
+	bool ranged = false;
+	std::vector<fb200_sample_range> range;
+	std::vector<uint32_t> errors;
+	std::vector<uint64_t> missing;
 };
 
 int reencode_fill(void *ctx, int32_t *pcm, unsigned long long values, const FileSeg *d_segs, cudaStream_t st)
 {
 	Reencode &R = *static_cast<Reencode *>(ctx);
-	return decoder_decode_into(R.dec, R.batch.data(), R.first_value.data(), (uint32_t)R.batch.size(), pcm, values, d_segs, 2 * (int)R.batch.size(), st);
+	const uint32_t n = (uint32_t)R.batch.size();
+	if(!R.ranged) return decoder_decode_into(R.dec, R.batch.data(), R.first_value.data(), n, pcm, values, d_segs, 2 * (int)n, st);
+	R.errors.resize(n);
+	R.missing.resize(n);
+	return decoder_decode_ranges_into(R.dec, R.range.data(), R.first_value.data(), n, pcm, values, d_segs, 2 * (int)n, st, R.errors.data(), R.missing.data());
 }
 
 int reencode_check(void *ctx, const uint8_t *d_md5, cudaStream_t st, std::vector<uint8_t> *keep)
@@ -156,17 +170,19 @@ int reencode_check(void *ctx, const uint8_t *d_md5, cudaStream_t st, std::vector
 	Reencode &R = *static_cast<Reencode *>(ctx);
 	const uint32_t n = (uint32_t)R.batch.size();
 	std::vector<uint8_t> md5(16 * (size_t)n);
-	std::vector<uint32_t> errors(n);
-	std::vector<uint64_t> missing(n);
-	FB_CUDA(cudaMemcpyAsync(md5.data(), d_md5, md5.size(), cudaMemcpyDeviceToHost, st));
-	const int rc = decoder_decode_verdicts(R.dec, R.batch.data(), n, st, errors.data(), missing.data());
-	if(rc != FB200_OK) return rc;
+	if(!R.ranged) {
+		R.errors.resize(n);
+		R.missing.resize(n);
+		FB_CUDA(cudaMemcpyAsync(md5.data(), d_md5, md5.size(), cudaMemcpyDeviceToHost, st));
+		const int rc = decoder_decode_verdicts(R.dec, R.batch.data(), n, st, R.errors.data(), R.missing.data());
+		if(rc != FB200_OK) return rc;
+	}
 	static const uint8_t zero[16] = {0};
 	R.status.assign(n, FB200_REENCODE_OK);
 	bool album = R.all_ok;
 	for(uint32_t i = 0; i < n; i++) {
-		const uint8_t *want = decoder_file_md5(R.dec, R.batch[i]);
-		if(errors[i] || missing[i]) R.status[i] = FB200_REENCODE_DAMAGED;
+		const uint8_t *want = R.ranged ? zero : decoder_file_md5(R.dec, R.batch[i]);
+		if(R.errors[i] || R.missing[i]) R.status[i] = FB200_REENCODE_DAMAGED;
 		else if(memcmp(want, zero, 16) != 0 && memcmp(want, md5.data() + 16 * (size_t)i, 16) != 0) R.status[i] = FB200_REENCODE_MD5_MISMATCH;
 		(*keep)[i] = R.status[i] == FB200_REENCODE_OK;
 		album &= R.status[i] == FB200_REENCODE_OK;
@@ -175,13 +191,15 @@ int reencode_check(void *ctx, const uint8_t *d_md5, cudaStream_t st, std::vector
 	return FB200_OK;
 }
 
-int reencode(fb200_encoder *e, fb200_decoder *dec, bool device, const uint32_t *files, uint32_t nfiles, const fb200_flac_reencode_options *opt,
-             const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *out, size_t out_capacity, uint64_t *frame_offsets, uint64_t *nframes,
-             fb200_flac_reencode_info *info, void *cuda_stream)
+// files[0 .. nfiles) whole (flac -f *.flac), or with ranges (files NULL), ranges[0 .. nfiles) (flac -f --skip --until *.flac)
+int reencode(fb200_encoder *e, fb200_decoder *dec, bool device, const uint32_t *files, const fb200_sample_range *ranges, uint32_t nfiles,
+             const fb200_flac_reencode_options *opt, const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *out, size_t out_capacity,
+             uint64_t *frame_offsets, uint64_t *nframes, fb200_flac_reencode_info *info, void *cuda_stream)
 {
-	if(!e || !dec || !files || !opt || !out || !nframes || !info) { set_error("a required pointer is NULL"); return FB200_ERR_INVALID; }
+	if(!e || !dec || (!files && !ranges) || !opt || !out || !nframes || !info) { set_error("a required pointer is NULL"); return FB200_ERR_INVALID; }
 	if(opt->reserved != 0) { set_error("fb200_flac_reencode_options.reserved must be 0"); return FB200_ERR_INVALID; }
-	if(nfiles == 0) { set_error("no files"); return FB200_ERR_INVALID; }
+	if(nfiles == 0 && !ranges) { set_error("no files"); return FB200_ERR_INVALID; }
+	if(ranges && (nfiles == 0 || nfiles >= 0x80000000u)) { set_error("invalid number of ranges %u", nfiles); return FB200_ERR_INVALID; }
 	if(!tags != !tag_offsets) { set_error("tags and tag_offsets must both be given or both be NULL"); return FB200_ERR_INVALID; }
 	uint32_t nbatch = 0;
 	int ddev = 0;
@@ -197,10 +215,25 @@ int reencode(fb200_encoder *e, fb200_decoder *dec, bool device, const uint32_t *
 	}
 	std::vector<uint8_t> seen(nbatch, 0);
 	for(uint32_t i = 0; i < nfiles; i++) {
-		const uint32_t f = files[i];
-		if(f >= nbatch) { set_error("files[%u] = %u, the batch has %u files", i, f, nbatch); return FB200_ERR_INVALID; }
-		if(seen[f]) { set_error("file %u is listed twice", f); return FB200_ERR_INVALID; }
-		seen[f] = 1;
+		const uint32_t f = ranges ? ranges[i].file : files[i];
+		if(ranges) {
+			// the checks of fb200_decode_files_ranges_*; a range past total_samples is the tool's "--until value is after end of input"
+			const fb200_sample_range &q = ranges[i];
+			if(f >= nbatch) { set_error("range %u: file %u of a batch of %u", i, f, nbatch); return FB200_ERR_INVALID; }
+			if(q.samples == 0) { set_error("range %u is empty", i); return FB200_ERR_INVALID; }
+			if(q.first_sample + q.samples < q.first_sample) { set_error("range %u: first_sample + samples overflows", i); return FB200_ERR_INVALID; }
+			const fb200_file_decode_info &I = decoder_file_info(dec, f);
+			if(I.status == FB200_FILE_OK && I.total_samples && q.first_sample + q.samples > I.total_samples) {
+				set_error("range %u: samples [%llu, %llu) of file %u, which has %llu", i, (unsigned long long)q.first_sample,
+				          (unsigned long long)(q.first_sample + q.samples), f, (unsigned long long)I.total_samples);
+				return FB200_ERR_INVALID;
+			}
+		}
+		else {
+			if(f >= nbatch) { set_error("files[%u] = %u, the batch has %u files", i, f, nbatch); return FB200_ERR_INVALID; }
+			if(seen[f]) { set_error("file %u is listed twice", f); return FB200_ERR_INVALID; }
+			seen[f] = 1;
+		}
 		const fb200_file_decode_info &I = decoder_file_info(dec, f);
 		if(I.status == FB200_FILE_OK && (I.channels != cfg.channels || I.bits_per_sample != cfg.bits_per_sample || I.sample_rate != cfg.sample_rate)) {
 			set_error("file %u is %u ch / %u bits / %u Hz, the encoder %u / %u / %u", f, I.channels, I.bits_per_sample, I.sample_rate, cfg.channels,
@@ -221,6 +254,7 @@ int reencode(fb200_encoder *e, fb200_decoder *dec, bool device, const uint32_t *
 	// ---- the host plan: each file's list, checked as the encoder checks it
 	Reencode R;
 	R.dec = dec;
+	R.ranged = ranges != nullptr;
 	RgRebuild rgr;
 	if(opt->replay_gain) {
 		R.rg = &rgr;
@@ -229,16 +263,21 @@ int reencode(fb200_encoder *e, fb200_decoder *dec, bool device, const uint32_t *
 	std::vector<uint32_t> listed;  // encoded file -> its place in files[]
 	std::vector<uint64_t> samples, moffs(1, 0);
 	std::vector<uint8_t> meta, region;
+	uint32_t region_of = ~0u;
 	uint64_t values = 0;
 	for(uint32_t i = 0; i < nfiles; i++) {
 		fb200_flac_reencode_info &O = info[i];
 		memset(&O, 0, sizeof O);
-		const uint32_t f = files[i];
+		const uint32_t f = ranges ? ranges[i].file : files[i];
 		const fb200_file_decode_info &I = decoder_file_info(dec, f);
 		if(I.status != FB200_FILE_OK) { fail(O, FB200_REENCODE_INPUT, "index status %u", I.status); continue; }
 		if(I.total_samples == 0) { fail(O, FB200_REENCODE_NO_TOTAL, "STREAMINFO has unknown total samples"); continue; }
+		const uint64_t length = ranges ? ranges[i].samples : I.samples;
 		int rc;
-		if((rc = decoder_file_metadata(dec, f, &region)) != FB200_OK) return rc;
+		if(region_of != f) {  // consecutive ranges of one file read its metadata once
+			if((rc = decoder_file_metadata(dec, f, &region)) != FB200_OK) return rc;
+			region_of = f;
+		}
 		if(region.size() >= 3 && memcmp(region.data(), "ID3", 3) == 0) { fail(O, FB200_REENCODE_INPUT, "input file has an ID3v2 tag"); continue; }  // main.c:1524
 		std::vector<Block> blocks;
 		std::vector<std::string> ent;
@@ -253,7 +292,7 @@ int reencode(fb200_encoder *e, fb200_decoder *dec, bool device, const uint32_t *
 		}
 		FileMeta M;
 		const char *why = input_blocks(region, &blocks);
-		if(!why) why = flac_input_metadata(std::move(blocks), *opt, ent, decoder_file_mask(dec, f), I.total_samples, I.sample_rate, &M);
+		if(!why) why = flac_input_metadata(std::move(blocks), *opt, ent, decoder_file_mask(dec, f), length, length == I.total_samples, I.sample_rate, &M);
 		if(why) { fail(O, FB200_REENCODE_METADATA, "%s", why); continue; }
 		std::vector<uint8_t> one;
 		put_file_metadata(M, one);
@@ -265,9 +304,10 @@ int reencode(fb200_encoder *e, fb200_decoder *dec, bool device, const uint32_t *
 		moffs.push_back(meta.size());
 		listed.push_back(i);
 		R.batch.push_back(f);
+		if(ranges) R.range.push_back(ranges[i]);
 		R.first_value.push_back(values);
-		samples.push_back(I.samples);
-		values += I.samples * I.channels;
+		samples.push_back(length);
+		values += length * I.channels;
 		if(opt->replay_gain) {
 			rg.bps.push_back(I.bits_per_sample);
 			rgr.files.push_back(std::move(M));
@@ -283,7 +323,7 @@ int reencode(fb200_encoder *e, fb200_decoder *dec, bool device, const uint32_t *
 
 	// ---- decode, MD5, verdicts and encode
 	PcmSource src;
-	src.data = reinterpret_cast<const uint8_t *>(files);  // not read: fill() provides the samples
+	src.data = reinterpret_cast<const uint8_t *>(info);  // not read: fill() provides the samples
 	src.bytes = 0;
 	src.rg = opt->replay_gain ? &rg : nullptr;
 	src.fill = reencode_fill;
@@ -307,8 +347,12 @@ int reencode(fb200_encoder *e, fb200_decoder *dec, bool device, const uint32_t *
 		uint32_t nbad = 0, first = 0;
 		for(uint32_t i = nfiles; i-- > 0;)
 			if(v[i].status != FB200_VERIFY_OK) { nbad++; first = i; }
-		set_error("%u file(s) failed verification; the first, files[%u] = %u: %s in frame %u", nbad, first, files[first],
-		          v[first].status == FB200_VERIFY_MISMATCH ? "sample mismatch" : "decoder error", v[first].frame_number);
+		if(ranges)
+			set_error("%u range(s) failed verification; the first, range %u of file %u: %s in frame %u", nbad, first, ranges[first].file,
+			          v[first].status == FB200_VERIFY_MISMATCH ? "sample mismatch" : "decoder error", v[first].frame_number);
+		else
+			set_error("%u file(s) failed verification; the first, files[%u] = %u: %s in frame %u", nbad, first, files[first],
+			          v[first].status == FB200_VERIFY_MISMATCH ? "sample mismatch" : "decoder error", v[first].frame_number);
 	}
 	return rc;
 }
@@ -323,12 +367,31 @@ int fb200_reencode_flac_files_host(fb200_encoder *e, fb200_decoder *dec, const u
                                    const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *out, size_t out_capacity, uint64_t *frame_offsets,
                                    uint64_t *nframes, fb200_flac_reencode_info *info)
 {
-	return reencode(e, dec, false, files, nfiles, opt, tags, tag_offsets, out, out_capacity, frame_offsets, nframes, info, nullptr);
+	if(!files) { set_error("a required pointer is NULL"); return FB200_ERR_INVALID; }
+	return reencode(e, dec, false, files, nullptr, nfiles, opt, tags, tag_offsets, out, out_capacity, frame_offsets, nframes, info, nullptr);
 }
 
 int fb200_reencode_flac_files_device(fb200_encoder *e, fb200_decoder *dec, const uint32_t *files, uint32_t nfiles, const fb200_flac_reencode_options *opt,
                                      const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *d_out, size_t out_capacity, uint64_t *d_frame_offsets,
                                      uint64_t *nframes, fb200_flac_reencode_info *info, void *cuda_stream)
 {
-	return reencode(e, dec, true, files, nfiles, opt, tags, tag_offsets, d_out, out_capacity, d_frame_offsets, nframes, info, cuda_stream);
+	if(!files) { set_error("a required pointer is NULL"); return FB200_ERR_INVALID; }
+	return reencode(e, dec, true, files, nullptr, nfiles, opt, tags, tag_offsets, d_out, out_capacity, d_frame_offsets, nframes, info, cuda_stream);
+}
+
+int fb200_reencode_flac_files_ranges_host(fb200_encoder *e, fb200_decoder *dec, const fb200_sample_range *ranges, uint32_t nranges,
+                                          const fb200_flac_reencode_options *opt, const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *out,
+                                          size_t out_capacity, uint64_t *frame_offsets, uint64_t *nframes, fb200_flac_reencode_info *info)
+{
+	if(!ranges) { set_error("ranges is NULL"); return FB200_ERR_INVALID; }
+	return reencode(e, dec, false, nullptr, ranges, nranges, opt, tags, tag_offsets, out, out_capacity, frame_offsets, nframes, info, nullptr);
+}
+
+int fb200_reencode_flac_files_ranges_device(fb200_encoder *e, fb200_decoder *dec, const fb200_sample_range *ranges, uint32_t nranges,
+                                            const fb200_flac_reencode_options *opt, const uint8_t *tags, const uint64_t *tag_offsets, uint8_t *d_out,
+                                            size_t out_capacity, uint64_t *d_frame_offsets, uint64_t *nframes, fb200_flac_reencode_info *info,
+                                            void *cuda_stream)
+{
+	if(!ranges) { set_error("ranges is NULL"); return FB200_ERR_INVALID; }
+	return reencode(e, dec, true, nullptr, ranges, nranges, opt, tags, tag_offsets, d_out, out_capacity, d_frame_offsets, nframes, info, cuda_stream);
 }

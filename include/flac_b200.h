@@ -332,6 +332,54 @@ int fb200_encode_pcm_files_device(fb200_encoder *enc, const uint8_t *d_data, con
                                   uint8_t *d_out, size_t out_capacity, uint64_t *d_frame_offsets, uint64_t *nframes,
                                   fb200_flac_file_info *files, void *cuda_stream);
 
+/* A sample range of one file of a batch: samples [first_sample, first_sample + samples) per channel (the ranged decode
+ * fb200_decode_files_ranges_* and the ranged encodes below). */
+typedef struct {
+	uint32_t file;            /* index into the batch (the indexed batch for .flac input, file_offsets' files for containers) */
+	uint32_t reserved;        /* 0 */
+	uint64_t first_sample;    /* per channel, from the file's start */
+	uint64_t samples;         /* per channel, >= 1 */
+} fb200_sample_range;
+
+/* ---- sample ranges of container files (flac [--skip] [--until] *.wav) ----
+ * fb200_encode_pcm_files_ranges_host / _device write one .flac per range of the probed files, in request order: range r's output is what flac --skip=<first_sample> --until=<first_sample + samples> writes for file
+ * ranges[r].file with the same options, and files[r] describes it (nranges records). A range may name any file any number of
+ * times, in any order, and ranges may overlap: k_pcm_unpack widens each range from its own first value, so every range gets its
+ * own copy. Everything else is as fb200_encode_pcm_files_*, with the range in place of the file:
+ *  - the SEEKTABLE template and the default padding's 20-minute threshold come from the range's length, not the declared count
+ *    (total_samples_to_encode, encode.c:2010, 2226);
+ *  - the channel-mask tag, MD5 (over the range's samples) and verify work per range; fb200_encoder_get_verify takes nranges
+ *    records; fb200_last_error counts ranges where it names a file of the encode;
+ *  - tags / tag_offsets hold nranges + 1 offsets: the -T entries are per range;
+ *  - with replay_gain the ranges are one album, as one tool invocation with one --skip / --until over several files.
+ * FB200_ERR_INVALID before any device work, naming the range and its file: the rules of fb200_encode_pcm_files_* for every file a
+ * range names (files no range names are not checked beyond their offsets); ranges NULL, nranges 0 or >= 2^31, a file index >= nfiles,
+ * samples 0, first_sample + samples overflowing; a range that starts past `declared` ("value of --skip exceeds input size") or ends
+ * past it ("--until value is after end of input").
+ * A data chunk cut short (samples < declared) follows the whole-file rule: the samples of the range that are present are encoded
+ * and the metadata is sized from the requested length. Known difference: a range that starts at or past the last sample present
+ * is FB200_ERR_INVALID, where the tool writes a stream without frames. */
+int fb200_encode_pcm_files_ranges_host(fb200_encoder *enc, const uint8_t *data, const uint64_t *file_offsets, uint32_t nfiles,
+                                       const fb200_pcm_file_info *info, const fb200_pcm_encode_options *opt,
+                                       const fb200_sample_range *ranges, uint32_t nranges, const uint8_t *tags, const uint64_t *tag_offsets,
+                                       uint8_t *out, size_t out_capacity, uint64_t *frame_offsets, uint64_t *nframes, fb200_flac_file_info *files);
+int fb200_encode_pcm_files_ranges_device(fb200_encoder *enc, const uint8_t *d_data, const uint64_t *file_offsets, uint32_t nfiles,
+                                         const fb200_pcm_file_info *info, const fb200_pcm_encode_options *opt,
+                                         const fb200_sample_range *ranges, uint32_t nranges, const uint8_t *tags, const uint64_t *tag_offsets,
+                                         uint8_t *d_out, size_t out_capacity, uint64_t *d_frame_offsets, uint64_t *nframes,
+                                         fb200_flac_file_info *files, void *cuda_stream);
+
+/* The flac tool's --skip / --until arithmetic, device-free (flac__utils_parse_skip_until_specification and
+ * flac__utils_canonicalize_skip_until_specification, utils.c:78-107, 326-398; main.c:1659-1670; encode.c:1003-1081, 2257-2303):
+ * skip NULL is no --skip, until NULL no --until (the tool's "-0"). Both take a sample count or [m]m:ss[.,]sss; seconds become
+ * samples as (int64_t)(seconds * sample_rate). skip may not be relative; until may: +N counts from skip, -N from the end, and any
+ * relative value that comes to 0 samples (+0, -0, -0:00.1 at a low rate) is the end of the stream. total_samples is the container's
+ * declared count or STREAMINFO total_samples; when it is 0 any until but the end is an error. Gives the range
+ * [*first_sample, *first_sample + *samples). Every case the tool rejects (a usage error or exit 1) is FB200_ERR_INVALID with the
+ * tool's message in fb200_last_error. Known difference: a range of 0 samples (skip equal to the length) is FB200_ERR_INVALID; the
+ * tool writes a stream without frames. */
+int fb200_skip_until(const char *skip, const char *until, uint32_t sample_rate, uint64_t total_samples, uint64_t *first_sample, uint64_t *samples);
+
 /* ---- re-encoding .flac files (flac -f [-S ..] [-P ..] [-T ..] [--replay-gain] *.flac) ----
  * fb200_reencode_flac_files_host / _device re-encode files[0 .. nfiles) of the batch left resident on `dec` by
  * fb200_decode_files_index into the .flac files the flac tool 1.5.0 writes from FLAC input, back to back in list order. Each listed
@@ -398,6 +446,34 @@ int fb200_reencode_flac_files_device(fb200_encoder *enc, fb200_decoder *dec, con
                                      const fb200_flac_reencode_options *opt, const uint8_t *tags, const uint64_t *tag_offsets,
                                      uint8_t *d_out, size_t out_capacity, uint64_t *d_frame_offsets, uint64_t *nframes,
                                      fb200_flac_reencode_info *info, void *cuda_stream);
+
+/* fb200_reencode_flac_files_ranges_host / _device: flac -f --skip=<first_sample> --until=<first_sample + samples> over sample ranges
+ * of the resident batch, one .flac per range in request order, info[r] (a FB200_REENCODE_* status) per range. A range may name any
+ * file any number of times, in any order, and ranges may overlap. The rules of fb200_reencode_flac_files_* hold per range, with the
+ * tool's changes for --skip / --until (encode.c:1003-1130, 1772-1930):
+ *  - MD5: the input's STREAMINFO MD5 is never compared (the tool zeroes it whenever --skip or --until is given), so MD5_MISMATCH
+ *    does not occur; the output's MD5 covers the range's samples.
+ *  - SEEKTABLE: the input's is kept (a template moved to the new frames) only when the range is the whole file (first_sample 0,
+ *    samples == total_samples) and seek_spacing_s is -1; otherwise it goes, and with -1 the "10s" template over the range's length
+ *    goes first.
+ *  - CUESHEET: kept when its lead-out equals the range's length, else dropped; track offsets are not moved (the tool's rule as
+ *    written).
+ *  - PADDING: the default's 20-minute threshold uses the range's length.
+ *  - STREAMINFO total_samples 0 gives NO_TOTAL for every range of that file.
+ *  - DAMAGED: a range with a damaged stretch among its candidate frames, or a sample no accepted frame covers, gets no bytes; frames
+ *    are accepted as fb200_decode_files_ranges_* accepts them, range_sees_its_frames included.
+ * FB200_ERR_INVALID before any device work: the call's checks of fb200_reencode_flac_files_* (a file listed twice excepted), ranges
+ * NULL, nranges 0 or >= 2^31, a file index out of range, samples 0, first_sample + samples overflowing, and a range past
+ * total_samples of a file whose index status is OK. The decoder's ranged path places every cropped frame straight into the
+ * encoder's input; samples never leave the device, and launches do not grow with nranges. Verify gives nranges records. */
+int fb200_reencode_flac_files_ranges_host(fb200_encoder *enc, fb200_decoder *dec, const fb200_sample_range *ranges, uint32_t nranges,
+                                          const fb200_flac_reencode_options *opt, const uint8_t *tags, const uint64_t *tag_offsets,
+                                          uint8_t *out, size_t out_capacity, uint64_t *frame_offsets, uint64_t *nframes,
+                                          fb200_flac_reencode_info *info);
+int fb200_reencode_flac_files_ranges_device(fb200_encoder *enc, fb200_decoder *dec, const fb200_sample_range *ranges, uint32_t nranges,
+                                            const fb200_flac_reencode_options *opt, const uint8_t *tags, const uint64_t *tag_offsets,
+                                            uint8_t *d_out, size_t out_capacity, uint64_t *d_frame_offsets, uint64_t *nframes,
+                                            fb200_flac_reencode_info *info, void *cuda_stream);
 
 /* ---- ReplayGain analysis of device PCM (the values flac --replay-gain and metaflac --add-replay-gain compute) ----
  * fb200_replaygain_device analyses int32 samples in device memory, in the layout fb200_decode_files_device writes: file f's
@@ -747,12 +823,6 @@ int fb200_decode_files_device(fb200_decoder *dec, int32_t *d_pcm, uint64_t pcm_c
  * No MD5 is computed (the reference turns MD5 checking off after a seek). The resident index is not changed: decode_files_*
  * afterwards returns what it returned before; the next index call replaces the batch for both. The per-frame status of
  * fb200_decoder_get_frame_status is left untouched. */
-typedef struct {
-	uint32_t file;            /* index into the indexed batch */
-	uint32_t reserved;        /* 0 */
-	uint64_t first_sample;    /* per channel, from the file's start */
-	uint64_t samples;         /* per channel, >= 1 */
-} fb200_sample_range;
 typedef struct {
 	uint32_t status;          /* FB200_FILE_* of the range's file; FB200_FILE_WIDTH as in fb200_decode_files_host */
 	uint32_t channels, bits_per_sample;
