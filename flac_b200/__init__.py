@@ -42,7 +42,7 @@ class EncoderConfig(C.Structure):
         ("min_residual_partition_order", C.c_uint32), ("max_residual_partition_order", C.c_uint32),
         ("num_apodizations", C.c_uint32), ("apodizations", Apodization * 32),
         ("disable_constant_subframes", C.c_int32), ("disable_fixed_subframes", C.c_int32),
-        ("disable_verbatim_subframes", C.c_int32), ("limit_min_bitrate", C.c_int32),
+        ("disable_verbatim_subframes", C.c_int32), ("limit_min_bitrate", C.c_int32), ("x86_avx2_fixed_guess", C.c_int32),
     ]
 
 
@@ -268,6 +268,8 @@ def lib():
     L.fb200_device_count.restype = C.c_int
     L.fb200_encoder_config_preset.restype = C.c_int
     L.fb200_encoder_config_preset.argtypes = [C.POINTER(EncoderConfig), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
+    L.fb200_host_x86_avx2_fixed_guess.restype = C.c_int
+    L.fb200_host_x86_avx2_fixed_guess.argtypes = []
     L.fb200_encoder_config_set_apodization.restype = C.c_int
     L.fb200_encoder_config_set_apodization.argtypes = [C.POINTER(EncoderConfig), C.c_char_p]
     L.fb200_window.restype = C.c_int
@@ -733,6 +735,12 @@ def preset(channels, bits_per_sample, sample_rate, compression_level, blocksize=
         else:
             setattr(cfg, k, v)
     return cfg
+
+
+def host_x86_avx2_fixed_guess():
+    """1 when libFLAC on this host guesses fixed orders with its x86 AVX2 routine (EncoderConfig.x86_avx2_fixed_guess for the
+    frames the flac tool writes here), else 0. Needs no GPU."""
+    return int(lib().fb200_host_x86_avx2_fixed_guess())
 
 
 def window(apodization, length):

@@ -186,6 +186,52 @@ __device__ __forceinline__ int fixed_best_order(const unsigned long long (&t)[5]
 	return guess;
 }
 
+// stream_encoder.c:4098-4103: the fixed order of a subframe is guessed by the _wide routine, the one libFLAC replaces with its
+// AVX2 version on x86-64 hosts that have AVX2. With EncK::x86_avx2_fixed_guess set, such subframes take that version's sums.
+__device__ __forceinline__ bool fixed_guess_avx2(const EncK &P, int bs, int sbps)
+{
+	return P.x86_avx2_fixed_guess && sbps < 28 && sbps + (int)ilog2_u32((uint32_t)(bs - (int)kMaxFixedOrder) * 17u) >= 32;
+}
+
+// Turns the C routine's fixed-guess sums into the x86 AVX2 routine's. te holds fixed.c:222-290's abs sums of the 0th .. 4th
+// differences over samples 4 .. bs-1 of the block x; afterwards it holds those of FLAC__fixed_compute_best_predictor_wide_intrin_avx2
+// (fixed_intrin_avx2.c:57-138). That routine splits the n = bs - 4 positions past the warm-up into four lanes: lane j = 0..3 sums
+// q = n / 4 positions from od_j = (j n) / 4 on, with positions op_j - 4 .. op_j - 1 (op_j = j q) as its difference history.
+// When n % 4 == 0 the two agree. Otherwise the n % 4 positions between two lanes and behind lane 3 are not summed, and the
+// first four positions of a lane whose history lies od_j - op_j (1 or 2) samples further back take their differences against
+// that history. So one thread corrects the sums by at most 11 positions' terms; they wrap on the way but end exact.
+__device__ __forceinline__ void fixed_guess_avx2_fixup(const int32_t *x, int bs, unsigned long long *te)
+{
+	const int n = bs - (int)kMaxFixedOrder, q = n >> 2;
+	if((n & 3) == 0) return;
+	const int32_t *d = x + kMaxFixedOrder;  // position p is d[p]
+	// adds (sign 1) or removes (sign -1) position p's terms; its predecessors m > k lie `back` samples further back. Subframe
+	// samples have at most 25 bits here (24-bit side channels), so every difference fits 32 bits.
+	auto terms = [&](int p, int k, int back, unsigned long long sign) {
+		const int32_t d0 = d[p], d1 = d[k < 1 ? p - 1 - back : p - 1], d2 = d[k < 2 ? p - 2 - back : p - 2];
+		const int32_t d3 = d[k < 3 ? p - 3 - back : p - 3], d4 = d[k < 4 ? p - 4 - back : p - 4];
+		const int32_t e1 = d0 - d1, e2 = d0 - 2 * d1 + d2, e3 = d0 - 3 * d1 + 3 * d2 - d3, e4 = d0 - 4 * d1 + 6 * d2 - 4 * d3 + d4;
+		te[0] += sign * abs_u32(d0);
+		te[1] += sign * abs_u32(e1);
+		te[2] += sign * abs_u32(e2);
+		te[3] += sign * abs_u32(e3);
+		te[4] += sign * abs_u32(e4);
+	};
+	int end = 2 * q;  // where the lane before lane j stops summing: lane 1 starts at od_1 = q, right behind lane 0
+	for(int j = 2; j <= 4; j++) {
+		const int od = j < 4 ? (j * n) >> 2 : n;
+		for(int p = end; p < od; p++) terms(p, kMaxFixedOrder, 0, ~0ull);  // between lanes j-1 and j, or behind lane 3
+		if(j == 4) break;
+		const int back = od - j * q;
+#pragma unroll 1
+		for(int k = 0; k < 4 && k < q && back; k++) {
+			terms(od + k, kMaxFixedOrder, 0, ~0ull);
+			terms(od + k, k, back, 1ull);
+		}
+		end = od + q;
+	}
+}
+
 // Partition order / Rice parameter search of one candidate (find_best_partition_order_ + set_partitioned_rice_,
 // stream_encoder.c:4701-5075), run by one whole warp. sums[0 .. 2^max_po) holds the candidate's |residual| sums per partition
 // at max_po and is overwritten; tmp holds at least 2^(max_po-1) entries. params_all receives order po's Rice parameters at

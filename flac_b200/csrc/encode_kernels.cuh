@@ -602,6 +602,10 @@ __global__ void __launch_bounds__(128) k_search(EncK P, const int32_t *__restric
 			if((tid & 31) == 0) atomicAdd(&S.te[k], te[k]);
 		}
 		__syncthreads();
+		if(fixed_guess_avx2(P, bs, sbps)) {
+			if(tid == 0) fixed_guess_avx2_fixup(x, bs, S.te);
+			__syncthreads();
+		}
 		const unsigned long long tt[5] = {S.te[0], S.te[1], S.te[2], S.te[3], S.te[4]};
 		float rbps[5];
 		const int guess = fixed_best_order(tt, bs, rbps);

@@ -13,6 +13,9 @@
 
 #include <map>
 #include <vector>
+#if defined(__x86_64__)
+#include <cpuid.h>
+#endif
 
 #include "fb200_internal.h"
 #include "flac_metadata.h"
@@ -232,6 +235,7 @@ static int build_geometry(fb200_encoder *e, int bs, Geometry **out)
 	k.sig_group = 0;
 	k.dis_const = c.disable_constant_subframes || (c.limit_min_bitrate && c.channels == 1);  // mono: the only channel is the last one
 	k.dis_fixed = c.disable_fixed_subframes; k.dis_verb = c.disable_verbatim_subframes;
+	k.x86_avx2_fixed_guess = c.x86_avx2_fixed_guess;
 	k.slot_stride = round_up((int)max_frame_bytes_for(c, (int)c.blocksize), 16);
 	k.slot_words = k.slot_stride / 4;
 	{
@@ -313,6 +317,8 @@ static int build_geometry(fb200_encoder *e, int bs, Geometry **out)
 			const int wps = 2;
 			const int gsz = k.nsig <= 4 ? k.nsig : 4;
 			const size_t need = rt ? search5_smem(bs, rt, gsz, wps, k.max_po, k.bps > 16) : 0;
+			// k_search5 has no x86_avx2_fixed_guess branch and needs none: the blocksizes it takes are multiples of 32 * rt, so
+			// bs - 4 is a multiple of 4, where the x86 AVX2 routine's fixed-guess sums equal the C routine's
 			if(rt && (ntl & (ntl - 1)) == 0 && k.max_po <= kMaxPartitionOrder && ((bs >> k.max_po) % rt) == 0 && need <= 200 * 1024 && 32 * wps * gsz <= 256) {
 				k.sig_group = k.nsig <= 4 ? 0 : gsz;
 				g.fast_search3 = rt;
@@ -607,6 +613,28 @@ int fb200_encoder_config_preset(fb200_encoder_config *cfg, uint32_t channels, ui
 	return FB200_OK;
 }
 
+// x86_cpu_info (cpu.c:151-200) as an x86-64 libFLAC built with AVX support runs it: cpuinfo.x86.avx2, and with it the AVX2
+// fixed-order guess (stream_encoder.c:1085-1090), needs AVX and OSXSAVE in CPUID leaf 1 ECX, the OS saving the XMM and YMM
+// state (XCR0 bits 1 and 2) and AVX2 in leaf 7 EBX. cpuinfo_x86 reads a leaf above the maximum as zeros.
+int fb200_host_x86_avx2_fixed_guess(void)
+{
+#if defined(__x86_64__)
+	const unsigned max_leaf = __get_cpuid_max(0, nullptr);
+	unsigned a, b, c, d;
+	if(max_leaf < 7) return 0;
+	__cpuid_count(1, 0, a, b, c, d);
+	if(!(c & (1u << 28)) || !(c & (1u << 27))) return 0;
+	unsigned xcr0_lo, xcr0_hi;
+	__asm__ volatile(".byte 0x0f, 0x01, 0xd0" : "=a"(xcr0_lo), "=d"(xcr0_hi) : "c"(0));  // XGETBV(0)
+	(void)a; (void)d; (void)xcr0_hi;
+	if((xcr0_lo & 6u) != 6u) return 0;
+	__cpuid_count(7, 0, a, b, c, d);
+	return (b & (1u << 5)) ? 1 : 0;
+#else
+	return 0;
+#endif
+}
+
 // FLAC__stream_encoder_set_apodization (stream_encoder.c:1940-2065): ';'-separated window names.
 // Unknown names are skipped; an empty result falls back to tukey(0.5); at most 32 windows.
 // Kept quirks: the '/' separators of the *_tukey(...) forms are searched with strchr from the
@@ -727,6 +755,7 @@ static int create_impl(const fb200_encoder_config *cfg_in, int device, uint32_t 
 	if(c.num_apodizations == 0 || c.num_apodizations > FB200_MAX_APODIZATIONS) { set_error("invalid number of apodizations"); return FB200_ERR_INVALID; }
 	for(uint32_t a = 0; a < c.num_apodizations; a++)
 		if(c.apodizations[a].type < FB200_APOD_TUKEY || c.apodizations[a].type > FB200_APOD_WELCH) { set_error("apodization type %d unknown", c.apodizations[a].type); return FB200_ERR_INVALID; }
+	if(c.x86_avx2_fixed_guess != 0 && c.x86_avx2_fixed_guess != 1) { set_error("invalid x86_avx2_fixed_guess %d (0 or 1)", c.x86_avx2_fixed_guess); return FB200_ERR_INVALID; }
 
 	int ndev = 0;
 	if(cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {

@@ -108,6 +108,7 @@ struct EncK {
 	int limit_min_bitrate;  // stream_encoder.c:3874: a frame must not consist of constant subframes only
 	int sig_group;       // k_search5: signals per CTA when a block's signals are split over several CTAs (0: one CTA per block)
 	const int *redo;     // search kernels, second pass of limit_min_bitrate: only blocks with redo[blk] != 0, only signals >= channels - 1
+	int x86_avx2_fixed_guess;  // fb200_encoder_config's: the general and tiled searches guess wide subframes' fixed order as x86 AVX2 libFLAC does
 };
 
 // ---- row layout shared by k_search5 and k_emit3: a signal lives in rows of R_T samples with a 36-word stride and one

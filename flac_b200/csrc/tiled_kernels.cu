@@ -175,6 +175,10 @@ __global__ void __launch_bounds__(kTiledThreads) k_search_tiled(EncK P, const in
 		eq = warp_and(eq);
 		if(lane == 0 && !eq) S.all_equal = 0;
 		__syncthreads();
+		if(fixed_guess_avx2(P, bs, sbps)) {
+			if(tid == 0) fixed_guess_avx2_fixup(g, bs, S.te);  // from global memory: the positions lie anywhere in the signal
+			__syncthreads();
+		}
 		const unsigned long long tt[5] = {S.te[0], S.te[1], S.te[2], S.te[3], S.te[4]};
 		float rbps[5];
 		const int guess = fixed_best_order(tt, bs, rbps);

@@ -94,6 +94,17 @@ typedef struct {
 	int32_t disable_fixed_subframes;        /* ..._disable_fixed_subframes */
 	int32_t disable_verbatim_subframes;     /* ..._disable_verbatim_subframes */
 	int32_t limit_min_bitrate;              /* set_limit_min_bitrate (stream_encoder.c:3874) */
+	/* Which fixed-order guess the encoder reproduces. libFLAC picks the fixed predictor order it tries from the abs sums of
+	 * each difference order. On x86-64 hosts with AVX2 it computes those sums for "wide" subframes (subframe bps < 28 and
+	 * bps + ilog2((blocksize - 4) * 17) >= 32, stream_encoder.c:4098-4103) with FLAC__fixed_compute_best_predictor_wide_intrin_avx2
+	 * (fixed_intrin_avx2.c:57-138) instead of its C routine. That routine splits the block into four lanes that skip up to 3
+	 * samples and read a few samples of history from the wrong place whenever blocksize - 4 is not a multiple of 4 (short last
+	 * blocks, odd blocksizes), so it can guess another order there, and the frames the flac tool writes on such a host differ.
+	 * 0 (default, written by fb200_encoder_config_preset): the C routine, what libFLAC computes everywhere else.
+	 * 1: the AVX2 routine for wide subframes, as libFLAC on an AVX2 host. fb200_host_x86_avx2_fixed_guess() tells which one the
+	 *    flac tool on this host uses. Full blocks of the standard blocksizes are identical in both modes.
+	 * Any other value fails fb200_encoder_create with FB200_ERR_INVALID. */
+	int32_t x86_avx2_fixed_guess;
 } fb200_encoder_config;
 
 typedef struct fb200_encoder fb200_encoder;
@@ -109,6 +120,11 @@ int fb200_device_count(void);                /* <0: FB200_ERR_CUDA */
  * (stream_encoder.c:117-140, 1873-1904) plus set_channels/bits_per_sample/sample_rate/blocksize. */
 int fb200_encoder_config_preset(fb200_encoder_config *cfg, uint32_t channels, uint32_t bits_per_sample,
                                 uint32_t sample_rate, uint32_t compression_level, uint32_t blocksize);
+
+/* 1 when libFLAC on this host would take its x86 AVX2 fixed-order guess (cpu.c:151-200: CPUID leaf 1 ECX has AVX and OSXSAVE,
+ * XGETBV(0) & 6 == 6, the maximum CPUID leaf is at least 7 and leaf 7 EBX has AVX2), else 0; always 0 on builds for other
+ * CPUs. Set fb200_encoder_config.x86_avx2_fixed_guess from it for the frames the flac tool writes on this host. Needs no GPU. */
+int fb200_host_x86_avx2_fixed_guess(void);
 
 /* FLAC__stream_encoder_set_apodization (stream_encoder.c:1940-2065): parse a ';'-separated
  * specification ("tukey(0.5);partial_tukey(2);gauss(0.2);hann" ...) into cfg->apodizations. */

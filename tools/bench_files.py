@@ -1,6 +1,6 @@
 """Batch-of-files encode benchmark (fb200_encode_files_host / _device).
 
-    python tools/bench_files.py [--steps 3] [--scale 1.0] [--only NAME] [--no-ref]
+    python tools/bench_files.py [--steps 3] [--scale 1.0] [--only NAME] [--no-ref] [--fixed-guess c|host]
 
 Per workload (ragged file lengths, seeded):
   device_*      fb200_encode_files_device, int32 PCM already on the device, host clock around the (synchronous) call
@@ -9,7 +9,10 @@ Per workload (ragged file lengths, seeded):
   md5_chain_mb_s  largest file's MD5 input bytes / device call time with MD5 on: the chain rate if the MD5 stream is the call's critical path
   tails_ms      device call over the files' tails alone (the general-path launches, one set per distinct tail length)
   ref_*         the reference with MD5 on, one encoder per file over every host thread
-  frames_equal / streaminfo_equal  every frame and every STREAMINFO (MD5 on) against the strict reference encoding each file alone
+  frames_equal / streaminfo_equal  every frame and every STREAMINFO (MD5 on) against the strict reference encoding each file alone,
+                dispatched as this host dispatches it
+  --fixed-guess host  encode with x86_avx2_fixed_guess = host_x86_avx2_fixed_guess() (the flac tool's frames on this host; default
+                c: the C routine), and time the device call and the tails with the field at 0 and at the host's value, alternating
   equal-length whole-block files, MD5 off: fb200_encode_files_device vs fb200_encode_device + set_file_blocks on the same input,
   alternating in one process (compaction + gather over the single-stream path)
 Prints one JSON line with the GPU's name and power limit (read-only nvidia-smi query)."""
@@ -61,18 +64,19 @@ def timed(fn, steps):
     return (time.perf_counter() - t) / steps
 
 
-def run(name, ch, bps, rate, level, bs, nfiles, lengths_fn, steps, scale, with_ref):
+def run(name, ch, bps, rate, level, bs, nfiles, lengths_fn, steps, scale, with_ref, fixed_guess):
     import torch
     lengths = np.maximum(lengths_fn(np.random.default_rng(7), scale, nfiles), 1).astype(np.uint64)
     total = int(lengths.sum())
     x = make_pcm(total, ch, bps, rate)
-    enc = flac_b200.Encoder(flac_b200.preset(ch, bps, rate, level, bs))
+    guess = flac_b200.host_x86_avx2_fixed_guess() if fixed_guess == "host" else 0
+    enc = flac_b200.Encoder(flac_b200.preset(ch, bps, rate, level, bs, x86_avx2_fixed_guess=guess))
     nfr, cap = enc.files_capacity(lengths)
     d_pcm = torch.from_numpy(x).cuda()
     d_out = torch.empty(cap, dtype=torch.uint8, device="cuda")
     d_off = torch.zeros(nfr + 1, dtype=torch.int64, device="cuda")
     nsamp = total * ch
-    r = {"workload": name, "files": nfiles, "samples_per_channel": total, "frames": nfr, "scale": scale}
+    r = {"workload": name, "files": nfiles, "samples_per_channel": total, "frames": nfr, "scale": scale, "x86_avx2_fixed_guess": guess}
 
     def dev(md5, lens=lengths):
         return enc.encode_files_device(d_pcm.data_ptr(), lens, d_out.data_ptr(), cap, d_off.data_ptr(), md5=md5)
@@ -105,6 +109,17 @@ def run(name, ch, bps, rate, level, bs, nfiles, lengths_fn, steps, scale, with_r
     tails = tails[tails > 0]
     r["distinct_tail_lengths"] = int(np.unique(tails).size)
     r["tails_ms"] = round(timed(lambda: dev(False, tails), steps) * 1e3, 2)
+    if fixed_guess == "host":
+        # the field at 0 and at the host's value, alternating: device call (MD5 off) and tails alone
+        enc_c = flac_b200.Encoder(flac_b200.preset(ch, bps, rate, level, bs))
+        ms = {"c": ([], []), "host": ([], [])}
+        for _ in range(5):
+            for e, m in ((enc_c, "c"), (enc, "host")):
+                for lens, acc in zip((lengths, tails), ms[m]):
+                    acc.append(round(timed(lambda: e.encode_files_device(d_pcm.data_ptr(), lens, d_out.data_ptr(), cap, d_off.data_ptr(), md5=False),
+                                           steps) * 1e3, 2))
+        enc_c.close()
+        r["fixed_guess_ms"] = {m: {"device_ms_md5_off": v[0], "tails_ms": v[1]} for m, v in ms.items()}
 
     # outputs of the last host call (MD5 on) against the reference, file by file
     out, off = h_out.numpy(), h_off.numpy()
@@ -181,13 +196,14 @@ def main():
     ap.add_argument("--scale", type=float, default=1.0, help="multiplies every file length")
     ap.add_argument("--only", default=None)
     ap.add_argument("--no-ref", action="store_true")
+    ap.add_argument("--fixed-guess", choices=("c", "host"), default="c", help="x86_avx2_fixed_guess: 0, or host_x86_avx2_fixed_guess()")
     a = ap.parse_args()
     name, power = gpu_info()
     res = []
     for w in WORKLOADS:
         if a.only and a.only != w[0]:
             continue
-        res.append(run(*w, a.steps, a.scale, not a.no_ref))
+        res.append(run(*w, a.steps, a.scale, not a.no_ref, a.fixed_guess))
     if not a.only:
         res.append(equal_length(a.steps))
     print(json.dumps({"gpu": name, "power_limit": power, "steps": a.steps, "results": res}))
