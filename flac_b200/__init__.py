@@ -33,6 +33,10 @@ class Apodization(C.Structure):
     _fields_ = [("type", C.c_int32), ("p", C.c_float), ("parts", C.c_int32), ("start", C.c_float), ("end", C.c_float)]
 
 
+class DebugAutocInfo(C.Structure):
+    _fields_ = [("nsec", C.c_uint32), ("lags", C.c_uint32), ("kernel_lags", C.c_uint32), ("lag_stride", C.c_uint32), ("route", C.c_int32)]
+
+
 class EncoderConfig(C.Structure):
     _fields_ = [
         ("channels", C.c_uint32), ("bits_per_sample", C.c_uint32), ("sample_rate", C.c_uint32), ("blocksize", C.c_uint32),
@@ -365,6 +369,9 @@ def lib():
     L.fb200_debug_lpc.argtypes = [C.c_int, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32,
                                   C.c_uint32, C.c_int, C.c_int, C.c_uint32, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_uint32)]
     L.fb200_debug_copy_plans.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.fb200_debug_copy_autoc.restype = C.c_int
+    L.fb200_debug_copy_autoc.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
+                                         C.POINTER(DebugAutocInfo)]
     if hasattr(L, "fb200_decoder_create"):
         L.fb200_decoder_create.restype = C.c_int
         L.fb200_decoder_create.argtypes = [C.POINTER(DecoderConfig), C.c_int, C.c_uint32, C.POINTER(C.c_void_p)]
@@ -1079,6 +1086,27 @@ class Encoder:
         n = (C.c_uint64 * 7)()
         _check(lib().fb200_encoder_get_profile(self._h, C.byref(ms), C.byref(n), 1 if reset else 0))
         return {name: (ms[i], int(n[i])) for i, name in enumerate(self.PROF_NAMES)}
+
+    STAGE_A_ROUTES = ("fused", "meta", "planar")
+
+    def debug_autoc(self, nblocks):
+        """Test hook fb200_debug_copy_autoc: what stage A left for the first nblocks full blocks of the last encode call. Returns
+        a dict: route ("fused" / "meta" / "planar"), lags (LPC lags), kernel_lags (lags each record holds), rows float64
+        [nsec, nblocks * nsig, lag_stride] (only [..., :kernel_lags] written), meta int32 [items, 2] (wasted bits, subframe bps),
+        sigor uint32 [items] (None off the fused route) and sections int32 [nsec, 5] (win_off, partial, data_len, part_size,
+        data_shift)."""
+        info = DebugAutocInfo()
+        _check(lib().fb200_debug_copy_autoc(self._h, nblocks, None, 0, None, None, None, 0, C.byref(info)))
+        nitems = nblocks * self.nsig
+        rows = np.full((info.nsec, nitems, info.lag_stride), np.nan)
+        meta = np.zeros((nitems, 2), dtype=np.int32)
+        sigor = np.zeros(nitems, dtype=np.uint32)
+        secs = np.zeros((info.nsec, 5), dtype=np.int32)
+        _check(lib().fb200_debug_copy_autoc(self._h, nblocks, rows.ctypes.data, rows.size, meta.ctypes.data, sigor.ctypes.data,
+                                            secs.ctypes.data, info.nsec, C.byref(info)))
+        route = self.STAGE_A_ROUTES[info.route]
+        return dict(route=route, lags=info.lags, kernel_lags=info.kernel_lags, rows=rows, meta=meta,
+                    sigor=sigor if route == "fused" else None, sections=secs)
 
     def debug_plans(self, nblocks):
         plans = (SubframePlan * (nblocks * self.nsig))()

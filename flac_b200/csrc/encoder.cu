@@ -105,6 +105,10 @@ struct fb200_encoder {
 	static constexpr int kStageAStreams = 4;
 	cudaStream_t s_as[kStageAStreams] = {};
 	bool slice_mode = false;
+	// the last call's full-block chunks (first block, blocks, StageA route) as stage A left them in workspace set 0 in slice
+	// mode: only fb200_debug_copy_autoc reads this
+	struct ChunkA { uint64_t first; uint32_t nb; int route; };
+	std::vector<ChunkA> chunks_a;
 	std::vector<cudaEvent_t> ev_ca;  // per chunk: stage A done
 	cudaEvent_t ev_fork = nullptr, ev_a[2] = {nullptr, nullptr}, ev_b[2] = {nullptr, nullptr};
 	bool ev_b_valid[2] = {false, false};
@@ -372,9 +376,9 @@ static void use_ws(fb200_encoder *e, int b, size_t off_blocks = 0)
 // What a chunk runs, decided once per chunk. k_autoc4, k_search5 and k_emit3 copy raw blocks of the caller's PCM with TMA, so
 // a chunk that starts off 16 bytes (the short last block behind an odd blocksize x channels) takes the planar kernels.
 enum class StageA {
-	fused,   // k_autoc4 on the caller's PCM collects the wasted-bits OR on the way; k_lpc derives wasted bits from it
-	meta,    // k_meta first (no LPC analysis, or loose mid-side: k_autoc4 reads the meta to skip the inactive pair), then k_autoc4
-	planar,  // k_prep's planar copy, then k_autoc3
+	fused = FB200_STAGE_A_FUSED,    // k_autoc4 on the caller's PCM collects the wasted-bits OR on the way; k_lpc derives wasted bits from it
+	meta = FB200_STAGE_A_META,      // k_meta first (no LPC analysis, or loose mid-side: k_autoc4 reads the meta to skip the inactive pair), then k_autoc4
+	planar = FB200_STAGE_A_PLANAR,  // k_prep's planar copy, then k_autoc3
 };
 enum class Kernel { fast, tiled, general };  // search: k_search5 / tiled / general; emit: k_emit3 / tiled / general + k_scan + k_gather
 struct Route { StageA a; Kernel search, emit; };
@@ -539,6 +543,7 @@ static int enqueue_chunk(fb200_encoder *e, size_t idx, const PipeChunk &c, const
 	use_ws(e, b, e->slice_mode ? (size_t)c.first : 0);
 	const int32_t *pcm = c.pcm ? c.pcm : d_pcm_base + (size_t)c.first * bs * ch;
 	const Route r = route_chunk(e, *g, pcm);
+	if(c.blocksize == e->cfg.blocksize) e->chunks_a.push_back(fb200_encoder::ChunkA{c.first, c.nb, (int)r.a});
 	if((rc = run_stage_a(e, *g, r.a, pcm, (int)c.nb, sa)) != FB200_OK) return rc;
 	cudaEvent_t done_a = e->ev_a[b];
 	if(e->slice_mode) {
@@ -564,6 +569,7 @@ static int enqueue_chunk(fb200_encoder *e, size_t idx, const PipeChunk &c, const
 static int fork_stage_a(fb200_encoder *e, uint64_t nblocks, cudaStream_t st)
 {
 	e->slice_mode = nblocks <= e->max_blocks;
+	e->chunks_a.clear();
 	FB_CUDA(cudaEventRecord(e->ev_fork, st));
 	for(int i = 0; i < (e->slice_mode ? fb200_encoder::kStageAStreams : 1); i++) FB_CUDA(cudaStreamWaitEvent(e->s_as[i], e->ev_fork, 0));
 	e->ev_b_valid[0] = e->ev_b_valid[1] = false;
@@ -775,8 +781,7 @@ static int create_impl(const fb200_encoder_config *cfg_in, int device, uint32_t 
 	}
 	e->nsig =(int)c.channels + ((c.channels == 2 && c.do_mid_side_stereo) ? 2 : 0);
 	{
-		const int lags = (int)c.max_lpc_order + 1;
-		e->lag_stride = lags <= 7 ? 7 : lags <= 9 ? 9 : lags <= 13 ? 13 : lags <= 17 ? 17 : 33;
+		e->lag_stride = (size_t)autoc_kernel_lags((int)c.max_lpc_order + 1);
 		size_t nsec = 0, nwin = 0;
 		for(uint32_t a = 0; a < c.num_apodizations; a++) {
 			nsec++; nwin++;
@@ -1803,6 +1808,52 @@ int fb200_debug_copy_plans(fb200_encoder *e, uint32_t nblocks, void *host_plans,
 	FB_CUDA(cudaDeviceSynchronize());
 	FB_CUDA(cudaMemcpy(host_plans, e->d_plans, (size_t)nblocks * e->nsig * sizeof(SubframePlan), cudaMemcpyDeviceToHost));
 	if(host_chan_assign) FB_CUDA(cudaMemcpy(host_chan_assign, e->d_chan_assign, nblocks * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+	return FB200_OK;
+}
+
+// stage A of the last call's full blocks (tests/test_gpu_autoc.py): reads the workspace slices the call's chunks left behind
+int fb200_debug_copy_autoc(fb200_encoder *e, uint32_t nblocks, double *autoc, size_t autoc_doubles, int32_t *meta, uint32_t *sigor,
+                           int32_t *sections, uint32_t max_sections, fb200_debug_autoc_info *info)
+{
+	if(!e || !info) return FB200_ERR_INVALID;
+	const auto it = e->geoms.find((int)e->cfg.blocksize);
+	if(nblocks == 0 || !e->slice_mode || it == e->geoms.end() || it->second.k.nwin == 0) {
+		set_error("fb200_debug_copy_autoc: the last call did not fit one workspace set, or its configuration computes no autocorrelation");
+		return FB200_ERR_INVALID;
+	}
+	const Geometry &g = it->second;
+	const size_t nsig = (size_t)e->nsig, nitems = (size_t)nblocks * nsig, ls = e->lag_stride, nsec = (size_t)g.k.nsec;
+	uint64_t covered = 0;
+	int route = -1;
+	for(const auto &c : e->chunks_a) {
+		if(covered >= nblocks) break;
+		if(c.first != covered || (route >= 0 && c.route != route)) {
+			set_error("fb200_debug_copy_autoc: the last call's full blocks are not consecutive chunks of one route");
+			return FB200_ERR_INVALID;
+		}
+		route = c.route;
+		covered += c.nb;
+	}
+	if(covered < nblocks) { set_error("fb200_debug_copy_autoc: the last call encoded %llu full blocks, not %u", (unsigned long long)covered, nblocks); return FB200_ERR_INVALID; }
+	info->nsec = (uint32_t)nsec; info->lags = (uint32_t)g.k.lags; info->kernel_lags = (uint32_t)autoc_kernel_lags(g.k.lags);
+	info->lag_stride = (uint32_t)ls; info->route = route;
+	if(!autoc) return FB200_OK;  // sizes only
+	if(!meta || !sigor || !sections || autoc_doubles < nsec * nitems * ls || max_sections < nsec) return FB200_ERR_INVALID;
+	static_assert(sizeof(SigMeta) == 2 * sizeof(int32_t) && sizeof(DevSection) == 5 * sizeof(int32_t), "the C ABI's layouts");
+	FB_CUDA(cudaSetDevice(e->device));
+	FB_CUDA(cudaDeviceSynchronize());
+	const size_t slice = e->max_nsec ? e->max_nsec : 1;
+	for(const auto &c : e->chunks_a) {
+		if(c.first >= nblocks) break;
+		const size_t n = (size_t)(c.nb < nblocks - c.first ? c.nb : nblocks - c.first) * nsig, cn = (size_t)c.nb * nsig, o = (size_t)c.first * nsig;
+		// use_ws: the chunk's records start at its first item's slice, section-major over the chunk's own items
+		const double *src = e->ws[0].d_autoc + o * slice * ls;
+		for(size_t sec = 0; sec < nsec; sec++)
+			FB_CUDA(cudaMemcpy(autoc + (sec * nitems + o) * ls, src + sec * cn * ls, n * ls * sizeof(double), cudaMemcpyDeviceToHost));
+		FB_CUDA(cudaMemcpy(meta + 2 * o, e->ws[0].d_meta + o, n * sizeof(SigMeta), cudaMemcpyDeviceToHost));
+		if(route == (int)StageA::fused) FB_CUDA(cudaMemcpy(sigor + o, e->ws[0].d_sigor + o, n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+	}
+	FB_CUDA(cudaMemcpy(sections, g.d_secs, nsec * sizeof(DevSection), cudaMemcpyDeviceToHost));
 	return FB200_OK;
 }
 

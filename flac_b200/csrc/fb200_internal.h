@@ -186,6 +186,7 @@ void launch_gather(const EncK &k, const uint8_t *slots, const uint32_t *bytes, c
 void launch_debug_log(const double *dx, double *dy, int n);
 void general_kernels_init(int device);  // raises the dynamic shared-memory limits once per device (never lowers them)
 // autoc_kernel.cu
+int autoc_kernel_lags(int lags);  // the LAGS instantiation k_autoc3 / k_autoc4 run for k.lags: values each record receives
 void launch_autoc3(const EncK &k, const int32_t *sig, const SigMeta *meta, const float *windows, const DevSection *secs, double *autoc, int nitems, cudaStream_t st);
 void autoc3_init(int device);
 void launch_autoc4(const EncK &k, const int32_t *pcm, const SigMeta *meta, const float *secwin, int secwin_stride, const DevSection *secs, double *autoc, int nitems, uint32_t *sigor, int or_sec, cudaStream_t st);

@@ -650,6 +650,26 @@ int fb200_encoder_get_profile(fb200_encoder *enc, double ms[FB200_PROF_KERNELS],
 /* Stage-level debug access used by the parity tests: the per-signal decisions (fb200::SubframePlan,
  * flac_b200/csrc/fb200_internal.h) and channel assignments of the most recent launch. */
 int fb200_debug_copy_plans(fb200_encoder *enc, uint32_t nblocks, void *host_plans, size_t plan_bytes, uint32_t *host_chan_assign);
+/* Stage A (the windowed FP64 autocorrelation) of the most recent encode call's first nblocks blocks, all of the configured
+ * blocksize, for tests that compare the kernels' sums with the reference's. The call's blocks must have fitted one workspace set
+ * (at most max_blocks_per_launch frames) and its full blocks must have taken one route; otherwise FB200_ERR_INVALID. info gets
+ * the section count, the LPC lag count, the lags the kernel computes and writes (kernel_lags), the record stride and the route
+ * (FB200_STAGE_A_*). With autoc == NULL nothing else is read. Otherwise, with item = block * nsig + signal:
+ *   autoc[(sec * nitems + item) * lag_stride + l], l < kernel_lags: the records as written -- on the fused route the sums of the
+ *     signal before its wasted bits are shifted out, on the others after; records of items with subframe bps 0 (the pair a loose
+ *     mid-side block does not code) are not written;
+ *   meta[2 * item], meta[2 * item + 1]: wasted bits and subframe bps;
+ *   sigor[item]: the OR of the signal's samples (fused route only; left untouched on the others);
+ *   sections[5 * sec ..]: window offset, partial, data_len, part_size and data_shift of each section (fb200::DevSection).
+ * The encode itself records only the route and block range of each chunk on the host for this: no launch, synchronisation or
+ * device allocation. */
+enum { FB200_STAGE_A_FUSED = 0, FB200_STAGE_A_META = 1, FB200_STAGE_A_PLANAR = 2 };
+typedef struct {
+	uint32_t nsec, lags, kernel_lags, lag_stride;
+	int32_t route;
+} fb200_debug_autoc_info;
+int fb200_debug_copy_autoc(fb200_encoder *enc, uint32_t nblocks, double *autoc, size_t autoc_doubles, int32_t *meta, uint32_t *sigor,
+                           int32_t *sections, uint32_t max_sections, fb200_debug_autoc_info *info);
 /* Verify tests: for the next fb200_encode_files_* call only, XOR xor_mask into a buffer the engine owns after the frames are
  * encoded and before they are verified. what = 0: byte b of frame a of file `file` in the encode scratch (the output is not
  * touched; a byte past the frame is left alone); what = 1: the value (sample a, channel b) of that file's int32 copy of the

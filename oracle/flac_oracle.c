@@ -398,7 +398,7 @@ void fo_config_set_apodization(fo_config *cfg, const char *spec)
 /* ------------------------------------------------------------------ LPC analysis */
 
 /* lpc.c:68-74 FLAC__lpc_window_data */
-static void window_data(const int32_t *in, const float *window, float *out, uint32_t data_len)
+void fo_window_data(const int32_t *in, const float *window, float *out, uint32_t data_len)
 {
 	uint32_t i;
 	for(i = 0; i < data_len; i++)
@@ -406,7 +406,7 @@ static void window_data(const int32_t *in, const float *window, float *out, uint
 }
 
 /* lpc.c:82-94 FLAC__lpc_window_data_partial */
-static void window_data_partial(const int32_t *in, const float *window, float *out, uint32_t data_len, uint32_t part_size, uint32_t data_shift)
+void fo_window_data_partial(const int32_t *in, const float *window, float *out, uint32_t data_len, uint32_t part_size, uint32_t data_shift)
 {
 	uint32_t i, j;
 	if((part_size + data_shift) < data_len) {
@@ -912,30 +912,34 @@ typedef struct {
 /* stream_encoder.c:4318-4392 apply_apodization_. Note the reference quirks kept here:
  * autoc_root copies only max_order entries (:4340) and the punch-out subtraction covers
  * only max_order entries (:4370-4371), so autoc[max_order] keeps the preceding partial
- * window's value. */
-static int apply_apodization(fo_encoder *e, apod_state *st, uint32_t blocksize, uint32_t max_order, const int32_t *signal)
+ * window's value. Each new autocorrelation has `lags` values (the reference's max_order + 1; fo_stage_a asks for as many
+ * as the CUDA kernel computes). Returns 2 when it computed a new autocorrelation, 1 for a punch-out, 0 for a skipped part. */
+static int apply_apodization(fo_encoder *e, apod_state *st, uint32_t blocksize, uint32_t max_order, uint32_t lags, const int32_t *signal)
 {
 	const fo_apodization *cur = &e->cfg.apodizations[st->a];
 	const float *win = e->window[st->a];
 
 	if(st->b == 1) {
-		window_data(signal, win, e->windowed, blocksize);
-		fo_autocorrelation(e->windowed, blocksize, max_order + 1, st->autoc);
+		fo_window_data(signal, win, e->windowed, blocksize);
+		fo_autocorrelation(e->windowed, blocksize, lags, st->autoc);
 		if(cur->type == FO_APOD_SUBDIVIDE_TUKEY) {
 			memcpy(st->autoc_root, st->autoc, max_order * sizeof(st->autoc[0]));
 			st->b++;
 		}
 		else
 			st->a++;
+		return 2;
 	}
 	else {
+		int made = 1;
 		if(blocksize / st->b <= FO_MAX_LPC_ORDER) {
 			next_subdivide_tukey(cur->parts, &st->a, &st->b, &st->c);
 			return 0;
 		}
 		if(!(st->c % 2)) {
-			window_data_partial(signal, win, e->windowed, blocksize, blocksize / st->b / 2, (st->c / 2 * blocksize) / st->b);
-			fo_autocorrelation(e->windowed, blocksize / st->b, max_order + 1, st->autoc);
+			fo_window_data_partial(signal, win, e->windowed, blocksize, blocksize / st->b / 2, (st->c / 2 * blocksize) / st->b);
+			fo_autocorrelation(e->windowed, blocksize / st->b, lags, st->autoc);
+			made = 2;
 		}
 		else {
 			uint32_t i;
@@ -943,8 +947,8 @@ static int apply_apodization(fo_encoder *e, apod_state *st, uint32_t blocksize, 
 				st->autoc[i] = st->autoc_root[i] - st->autoc[i];
 		}
 		next_subdivide_tukey(cur->parts, &st->a, &st->b, &st->c);
+		return made;
 	}
-	return 1;
 }
 
 /* stream_encoder.c:4376-4391 (the tail of apply_apodization_) and :4220-4260 + 4591-4599 (process_subframe_'s order and
@@ -1068,7 +1072,7 @@ static uint32_t process_subframe(fo_encoder *e, const int32_t *signal, uint32_t 
 					st.a = 0; st.b = 1; st.c = 0;
 					while(st.a < cfg->num_apodizations) {
 						size_t n, i;
-						if(!apply_apodization(e, &st, blocksize, max_lpc_order, signal))
+						if(!apply_apodization(e, &st, blocksize, max_lpc_order, max_lpc_order + 1, signal))
 							continue;
 						n = fo_lpc_candidates(st.autoc, max_lpc_order, subframe_bps, blocksize, cfg, e->lpc_cands);
 						for(i = 0; i < n; i++) {
@@ -1334,27 +1338,17 @@ static void ensure_windows(fo_encoder *e, uint32_t blocksize)
 	e->win_blocksize = blocksize;
 }
 
-/* stream_encoder.c:3747-4043 process_subframes_ + :3435-3480 process_frame_ (pad, CRC-16) */
-size_t fo_encode_frame(fo_encoder *e, const int32_t *interleaved, uint32_t blocksize, uint32_t frame_number,
-                       uint8_t *out, size_t out_cap, fo_frame_plan *plan_out)
+/* stream_encoder.c:3777-3867: the channels (e->chan), mid and side (e->sig[2], e->sig[3]) when the block codes them, the
+ * loose mid-side decision, and each coded signal's wasted bits shifted out in place with its subframe bps */
+static void form_signals(fo_encoder *e, const int32_t *interleaved, uint32_t blocksize, int *do_independent_out, int *do_mid_side_out,
+                         uint32_t *channel_assignment, uint32_t wasted[], uint32_t sbps[], uint32_t ms_wasted[2], uint32_t ms_bps[2])
 {
 	const fo_config *cfg = &e->cfg;
 	const uint32_t ch = cfg->channels, bps = cfg->bits_per_sample;
-	uint32_t min_po = cfg->min_residual_partition_order, max_po;
-	int do_independent, do_mid_side, all_constant = 1, disable_constant = cfg->disable_constant_subframes;
-	uint32_t channel_assignment = 0, c, i;
-	fo_subframe_plan plans[FO_MAX_CHANNELS], ms_plans[2];
-	uint32_t bits[FO_MAX_CHANNELS], ms_bits[2] = {0, 0};
-	uint32_t wasted[FO_MAX_CHANNELS], sbps[FO_MAX_CHANNELS], ms_wasted[2], ms_bps[2];
-	bitw bw;
+	int do_independent, do_mid_side;
+	uint32_t c, i;
 
-	if(blocksize == 0 || blocksize > cfg->blocksize) return 0;
-	ensure_windows(e, blocksize);
-
-	max_po = max_rice_partition_order_from_blocksize(blocksize);
-	max_po = MINU(max_po, cfg->max_residual_partition_order);
-	min_po = MINU(min_po, max_po);
-
+	*channel_assignment = 0;
 	for(c = 0; c < ch; c++)
 		for(i = 0; i < blocksize; i++)
 			e->chan[c][i] = interleaved[(size_t)i * ch + c];
@@ -1368,8 +1362,8 @@ size_t fo_encode_frame(fo_encoder *e, const int32_t *interleaved, uint32_t block
 				sumAbsLR += (uint64_t)(abs(pl) + abs(pr));
 				sumAbsMS += (uint64_t)(abs((pl + pr) >> 1) + abs(pl - pr));
 			}
-			if(sumAbsLR < sumAbsMS) { do_independent = 1; do_mid_side = 0; channel_assignment = 0; }
-			else { do_independent = 0; do_mid_side = 1; channel_assignment = 3; }
+			if(sumAbsLR < sumAbsMS) { do_independent = 1; do_mid_side = 0; *channel_assignment = 0; }
+			else { do_independent = 0; do_mid_side = 1; *channel_assignment = 3; }
 		}
 		else { do_independent = 1; do_mid_side = 1; }
 	}
@@ -1397,6 +1391,90 @@ size_t fo_encode_frame(fo_encoder *e, const int32_t *interleaved, uint32_t block
 			ms_bps[c] = bps - w + (c == 0 ? 0 : 1);
 		}
 	}
+	*do_independent_out = do_independent;
+	*do_mid_side_out = do_mid_side;
+}
+
+int fo_stage_a(fo_encoder *e, const int32_t *interleaved, uint32_t nblocks, uint32_t lags, uint32_t lag_stride, int unshifted,
+               double *rows, size_t rows_cap, int32_t *meta, uint32_t *sigor)
+{
+	const fo_config *cfg = &e->cfg;
+	const uint32_t bs = cfg->blocksize, ch = cfg->channels, nsig = ch + (cfg->do_mid_side ? 2u : 0u);
+	const size_t nitems = (size_t)nblocks * nsig;
+	uint32_t max_order, nsec = 0, a, b, blk, s, i;
+	int32_t *x;
+
+	if(cfg->max_lpc_order == 0 || bs < 2 || lags < 1 || lags > FO_MAX_LPC_ORDER + 1 || lag_stride < lags) return -1;
+	for(a = 0; a < cfg->num_apodizations; a++) {
+		nsec++;
+		if(cfg->apodizations[a].type == FO_APOD_SUBDIVIDE_TUKEY)
+			for(b = 2; b <= (uint32_t)cfg->apodizations[a].parts; b++)
+				if(bs / b > FO_MAX_LPC_ORDER) nsec += b == 2 ? 2 : b;
+	}
+	if((size_t)nsec * nitems * lag_stride > rows_cap) return -1;
+	max_order = cfg->max_lpc_order >= bs ? bs - 1 : cfg->max_lpc_order;
+	x = (int32_t *)malloc(sizeof(int32_t) * bs);
+	if(!x) return -1;
+	memset(rows, 0, sizeof(double) * (size_t)nsec * nitems * lag_stride);
+	ensure_windows(e, bs);
+	for(blk = 0; blk < nblocks; blk++) {
+		int do_independent, do_mid_side;
+		uint32_t ca, wasted[FO_MAX_CHANNELS], sbps[FO_MAX_CHANNELS], ms_wasted[2], ms_bps[2];
+		form_signals(e, interleaved + (size_t)blk * bs * ch, bs, &do_independent, &do_mid_side, &ca, wasted, sbps, ms_wasted, ms_bps);
+		for(s = 0; s < nsig; s++) {
+			const size_t item = (size_t)blk * nsig + s;
+			const int ms = s >= ch;
+			const int32_t *sig = ms ? e->sig[2 + s - ch] : e->chan[s];
+			const uint32_t w = ms ? ms_wasted[s - ch] : wasted[s];
+			uint32_t o = 0, sec = 0;
+			apod_state st;
+			meta[2 * item] = 0;
+			meta[2 * item + 1] = 0;
+			sigor[item] = 0;
+			if(!(ms ? do_mid_side : do_independent)) continue;
+			meta[2 * item] = (int32_t)w;
+			meta[2 * item + 1] = (int32_t)(ms ? ms_bps[s - ch] : sbps[s]);
+			for(i = 0; i < bs; i++) {
+				x[i] = (int32_t)((uint32_t)sig[i] << w);  /* the signal before get_wasted_bits shifted its w zero bits out */
+				o |= (uint32_t)x[i];
+			}
+			sigor[item] = o;
+			memset(&st, 0, sizeof st);
+			st.b = 1;
+			while(st.a < cfg->num_apodizations)
+				if(apply_apodization(e, &st, bs, max_order, lags, unshifted ? x : sig) == 2) {
+					if(sec == nsec) { free(x); return -1; }
+					memcpy(rows + ((size_t)sec * nitems + item) * lag_stride, st.autoc, lags * sizeof(double));
+					sec++;
+				}
+		}
+	}
+	free(x);
+	return (int)nsec;
+}
+
+/* stream_encoder.c:3747-4043 process_subframes_ + :3435-3480 process_frame_ (pad, CRC-16) */
+size_t fo_encode_frame(fo_encoder *e, const int32_t *interleaved, uint32_t blocksize, uint32_t frame_number,
+                       uint8_t *out, size_t out_cap, fo_frame_plan *plan_out)
+{
+	const fo_config *cfg = &e->cfg;
+	const uint32_t ch = cfg->channels;
+	uint32_t min_po = cfg->min_residual_partition_order, max_po;
+	int do_independent, do_mid_side, all_constant = 1, disable_constant = cfg->disable_constant_subframes;
+	uint32_t channel_assignment = 0, c;
+	fo_subframe_plan plans[FO_MAX_CHANNELS], ms_plans[2];
+	uint32_t bits[FO_MAX_CHANNELS], ms_bits[2] = {0, 0};
+	uint32_t wasted[FO_MAX_CHANNELS], sbps[FO_MAX_CHANNELS], ms_wasted[2], ms_bps[2];
+	bitw bw;
+
+	if(blocksize == 0 || blocksize > cfg->blocksize) return 0;
+	ensure_windows(e, blocksize);
+
+	max_po = max_rice_partition_order_from_blocksize(blocksize);
+	max_po = MINU(max_po, cfg->max_residual_partition_order);
+	min_po = MINU(min_po, max_po);
+
+	form_signals(e, interleaved, blocksize, &do_independent, &do_mid_side, &channel_assignment, wasted, sbps, ms_wasted, ms_bps);
 	if(plan_out) memset(plan_out, 0, sizeof *plan_out);
 
 	if(do_independent) {

@@ -111,6 +111,9 @@ void fo_window_tukey(float *window, int32_t L, float p);
 int fo_window(const fo_apodization *a, float *window, int32_t L);     /* any FO_APOD_* ; 0 on unknown type */
 void fo_config_set_apodization(fo_config *cfg, const char *spec);     /* FLAC__stream_encoder_set_apodization */
 void fo_autocorrelation(const float *data, uint32_t data_len, uint32_t lag, double *autoc);
+void fo_window_data(const int32_t *in, const float *window, float *out, uint32_t data_len);  /* lpc.c:68-74 */
+void fo_window_data_partial(const int32_t *in, const float *window, float *out, uint32_t data_len, uint32_t part_size,
+                            uint32_t data_shift);                                            /* lpc.c:82-94 */
 void fo_lp_coefficients(const double *autoc, uint32_t *max_order, float lp_coeff[][FO_MAX_LPC_ORDER], double *error);
 uint32_t fo_best_order(const double *lpc_error, uint32_t max_order, uint32_t total_samples, uint32_t overhead_bits_per_order);
 int fo_quantize_coefficients(const float *lp_coeff, uint32_t order, uint32_t precision, int32_t *qlp_coeff, int *shift);
@@ -120,6 +123,19 @@ uint16_t fo_crc16(const uint8_t *data, size_t len);
 uint64_t fo_max_prediction_value_before_shift(uint32_t subframe_bps, const int32_t *qlp, uint32_t order);
 uint32_t fo_max_residual_bps(uint32_t subframe_bps, const int32_t *qlp, uint32_t order, int lp_quantization);
 uint32_t fo_silog2(int64_t v);
+
+/* What the CUDA encoder's stage A must produce for nblocks whole blocks of cfg.blocksize samples (interleaved int32 PCM), per
+ * (block, signal) item -- signals are the channels, then mid and side when the configuration codes mid-side, formed as
+ * stream_encoder.c:3777-3867 forms them:
+ *   meta[2 * item], meta[2 * item + 1]: wasted bits and subframe bps; both 0 for the pair a loose mid-side block does not code;
+ *   sigor[item]: the OR of the signal's samples before its wasted bits are shifted out (0 for an uncoded pair);
+ *   rows[(sec * nitems + item) * lag_stride + l], l < lags: the autocorrelation of every section apply_apodization_ computes
+ *   (:4318-4392), in the order it computes them; punch-out differences are not sections. unshifted = 1: rows of the signal
+ *   before its wasted bits are shifted out. An uncoded pair's rows are 0.
+ * lags may exceed max_lpc_order + 1 (the kernels compute a fixed number of lags): every lag is the same ascending sum.
+ * Returns the number of sections, -1 on bad arguments or when rows_cap (doubles) is too small. */
+int fo_stage_a(fo_encoder *e, const int32_t *interleaved, uint32_t nblocks, uint32_t lags, uint32_t lag_stride, int unshifted,
+               double *rows, size_t rows_cap, int32_t *meta, uint32_t *sigor);
 
 /* One LPC candidate of one apodization, in the order process_subframe_ evaluates them (stream_encoder.c:4220-4260, 4591-4599). */
 enum { FO_LPC_QUANTIZED = 0, FO_LPC_SHIFT_TOO_SMALL = 1, FO_LPC_CMAX_ZERO = 2, FO_LPC_DONT_EVEN_TRY = 3 };

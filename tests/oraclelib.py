@@ -98,6 +98,11 @@ def lib():
         L.fo_window.restype = C.c_int
         L.fo_window.argtypes = [C.POINTER(Apod), C.c_void_p, C.c_int32]
         L.fo_autocorrelation.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
+        L.fo_window_data.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
+        L.fo_window_data_partial.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32]
+        L.fo_stage_a.restype = C.c_int
+        L.fo_stage_a.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p,
+                                 C.c_void_p]
         L.fo_lpc_candidates.restype = C.c_size_t
         L.fo_lpc_candidates.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(Config), C.POINTER(LpcCand)]
         L.fo_lpc_estimate.restype = C.c_uint32
@@ -128,6 +133,32 @@ def window(apod, length):
     out = np.empty(length, dtype=np.float32)
     if not lib().fo_window(C.byref(apod), out.ctypes.data, length):
         raise ValueError("unknown apodization type")
+    return out
+
+
+def autocorrelation(data, lags):
+    """fo_autocorrelation: lags sums of the float32 data, each in ascending sample order."""
+    d = np.ascontiguousarray(data, dtype=np.float32)
+    out = np.zeros(lags, dtype=np.float64)
+    lib().fo_autocorrelation(d.ctypes.data, d.size, lags, out.ctypes.data)
+    return out
+
+
+def window_data(x, win):
+    """fo_window_data: x[i] * win[i] in float (lpc.c:68-74)."""
+    x = np.ascontiguousarray(x, dtype=np.int32)
+    w = np.ascontiguousarray(win, dtype=np.float32)
+    out = np.zeros(x.size, dtype=np.float32)
+    lib().fo_window_data(x.ctypes.data, w.ctypes.data, out.ctypes.data, x.size)
+    return out
+
+
+def window_data_partial(x, win, part_size, data_shift, init=0.0):
+    """fo_window_data_partial over data_len = len(x) (lpc.c:82-94); entries it does not write keep `init`."""
+    x = np.ascontiguousarray(x, dtype=np.int32)
+    w = np.ascontiguousarray(win, dtype=np.float32)
+    out = np.full(x.size, init, dtype=np.float32)
+    lib().fo_window_data_partial(x.ctypes.data, w.ctypes.data, out.ctypes.data, x.size, part_size, data_shift)
     return out
 
 
@@ -181,6 +212,27 @@ class Encoder:
         if ln == 0:
             raise RuntimeError("fo_encode_frame failed")
         return (out[:ln].tobytes(), plan) if want_plan else out[:ln].tobytes()
+
+    def stage_a(self, pcm, lags, lag_stride=None, unshifted=False):
+        """fo_stage_a on whole blocks of cfg.blocksize: (rows float64 [nsec, items, lag_stride], meta int32 [items, 2], sigor
+        uint32 [items]), item = block * nsig + signal."""
+        pcm = np.ascontiguousarray(pcm, dtype=np.int32)
+        n, ch = pcm.shape
+        bs = self.cfg.blocksize
+        assert n % bs == 0 and ch == self.cfg.channels
+        nb = n // bs
+        nsig = ch + (2 if self.cfg.do_mid_side else 0)
+        lag_stride = lag_stride or lags
+        nsec_max = sum(1 + (sum(b if b > 2 else 2 for b in range(2, a.parts + 1)) if a.type == 1 else 0)
+                       for a in self.cfg.apodizations[:self.cfg.num_apodizations])
+        rows = np.zeros(nsec_max * nb * nsig * lag_stride, dtype=np.float64)
+        meta = np.zeros((nb * nsig, 2), dtype=np.int32)
+        sigor = np.zeros(nb * nsig, dtype=np.uint32)
+        nsec = lib().fo_stage_a(self.h, pcm.ctypes.data, nb, lags, lag_stride, int(unshifted), rows.ctypes.data, rows.size,
+                                meta.ctypes.data, sigor.ctypes.data)
+        if nsec < 0:
+            raise ValueError("fo_stage_a: bad arguments")
+        return rows[:nsec * nb * nsig * lag_stride].reshape(nsec, nb * nsig, lag_stride), meta, sigor
 
     def encode_stream(self, pcm):
         pcm = np.ascontiguousarray(pcm, dtype=np.int32)
