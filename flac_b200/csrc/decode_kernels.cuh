@@ -28,14 +28,9 @@
 #include <type_traits>
 
 #include "fb200_internal.h"
+#include "flac_frame.cuh"
 
 namespace fb200 {
-
-enum : uint32_t {
-	DEC_OK = 0, DEC_BAD_SYNC = 1, DEC_BAD_HEADER = 2, DEC_CRC8 = 3, DEC_UNSUPPORTED = 4, DEC_PARSE = 5,
-	DEC_LENGTH = 6, DEC_CRC16 = 7, DEC_MISMATCH = 8, DEC_RANGE = 9,
-	DEC_WRONG_FRAME = 10  // verify: the coded frame number or blocksize is not this frame's (FB200_VERIFY_WRONG_FRAME)
-};
 
 struct DecK {
 	int channels, bps, sample_rate, blocksize;  // STREAMINFO facts
@@ -211,32 +206,8 @@ __global__ void __launch_bounds__(256) k_dec_scan(const uint8_t *__restrict__ da
 	const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
 	for(unsigned long long p = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; p + 6 <= n; p += stride) {
 		if(data[p] != 0xFF || (data[p + 1] & 0xFE) != 0xF8) continue;
-		const uint8_t *h = data + p;
-		const unsigned long long avail = n - p;
-		const uint32_t variable = h[1] & 1, bs_code = h[2] >> 4, sr_code = h[2] & 15, ca_code = h[3] >> 4, bps_code = (h[3] >> 1) & 7;
-		if((h[3] & 1) || bs_code == 0 || sr_code == 15 || ca_code > 10 || bps_code == 3) continue;
-		uint32_t pos = 4;
-		const uint32_t first = h[pos++];
-		int nb;
-		if(!(first & 0x80)) nb = 0;
-		else if((first & 0xE0) == 0xC0) nb = 1;
-		else if((first & 0xF0) == 0xE0) nb = 2;
-		else if((first & 0xF8) == 0xF0) nb = 3;
-		else if((first & 0xFC) == 0xF8) nb = 4;
-		else if((first & 0xFE) == 0xFC) nb = 5;
-		else if(first == 0xFE && variable) nb = 6;
-		else continue;
-		const uint32_t hl = pos + nb + (bs_code == 6 ? 1 : bs_code == 7 ? 2 : 0) + (sr_code == 12 ? 1 : sr_code >= 13 ? 2 : 0);
-		if(hl + 1 > avail) continue;
-		bool ok = true;
-		for(int k = 0; k < nb; k++) ok = ok && (h[pos + k] & 0xC0) == 0x80;
-		if(!ok) continue;
-		uint32_t crc = 0;
-		for(uint32_t b = 0; b < hl; b++) {
-			crc ^= h[b];
-			for(int j = 0; j < 8; j++) crc = (crc & 0x80u) ? ((crc << 1) ^ 0x07u) & 0xffu : (crc << 1) & 0xffu;
-		}
-		if(crc != h[hl]) continue;
+		FrameHeader fh;
+		if(parse_frame_header(data + p, n - p, 0, 0, fh).status != DEC_OK) continue;
 		const unsigned slot = atomicAdd(count, 1u);
 		if(slot < cap) cand[slot] = p;
 	}
@@ -255,77 +226,14 @@ __global__ void __launch_bounds__(128) k_dec_walk(DecK P, const uint8_t *__restr
 	M.status = DEC_OK; M.blocksize = 0; M.channel_assignment = 0; M.channels = 0; M.frame_bytes = 0; M.frame_number_lo = 0; M.variable = 0; M.sample_rate = 0; M.max_order = 0;
 #pragma unroll
 	for(int c = 0; c < FB200_MAX_CHANNELS; c++) M.sub_bit[c] = 0;
-	if(len < 6) { M.status = DEC_LENGTH; meta[f] = M; return; }
+	FrameHeader fh;
+	const FrameHeaderRead hr = parse_frame_header(frames + off, len, (uint32_t)P.sample_rate, (uint32_t)P.bps, fh);
+	if(hr.status != DEC_OK) { M.status = hr.status; meta[f] = M; return; }
+	const uint32_t blocksize = fh.blocksize, ca = fh.ca, channels = fh.channels, bps = fh.bps;
 	BitRd br;
-	br.init(frames + off, len, 0);
-	const uint32_t start = br.pos;
-
-	// ---- frame header (stream_decoder.c:2624-2947)
-	if(br.get(14) != 0x3ffe) { M.status = DEC_BAD_SYNC; meta[f] = M; return; }
-	if(br.get(1) != 0) { M.status = DEC_BAD_HEADER; meta[f] = M; return; }
-	const uint32_t variable = br.get(1);
-	const uint32_t bs_code = br.get(4), sr_code = br.get(4), ca_code = br.get(4), bps_code = br.get(3);
-	if(br.get(1) != 0) { M.status = DEC_BAD_HEADER; meta[f] = M; return; }
-	unsigned long long number = 0;
-	{   // UTF-8 coded frame/sample number
-		const uint32_t first = br.get(8);
-		int n;
-		if(!(first & 0x80)) { n = 0; number = first; }
-		else if((first & 0xE0) == 0xC0) { n = 1; number = first & 0x1F; }
-		else if((first & 0xF0) == 0xE0) { n = 2; number = first & 0x0F; }
-		else if((first & 0xF8) == 0xF0) { n = 3; number = first & 0x07; }
-		else if((first & 0xFC) == 0xF8) { n = 4; number = first & 0x03; }
-		else if((first & 0xFE) == 0xFC) { n = 5; number = first & 0x01; }
-		else if(first == 0xFE && variable) { n = 6; number = 0; }
-		else { M.status = DEC_BAD_HEADER; meta[f] = M; return; }
-		for(int k = 0; k < n; k++) {
-			const uint32_t b = br.get(8);
-			if((b & 0xC0) != 0x80) { M.status = DEC_BAD_HEADER; meta[f] = M; return; }
-			number = (number << 6) | (b & 0x3F);
-		}
-	}
-	uint32_t blocksize;
-	switch(bs_code) {
-		case 0: M.status = DEC_BAD_HEADER; meta[f] = M; return;
-		case 1: blocksize = 192; break;
-		case 2: case 3: case 4: case 5: blocksize = 576u << (bs_code - 2); break;
-		case 6: blocksize = br.get(8) + 1; break;
-		case 7: blocksize = br.get(16) + 1; break;
-		default: blocksize = 256u << (bs_code - 8); break;
-	}
-	uint32_t rate = (uint32_t)P.sample_rate;
-	switch(sr_code) {
-		case 0: break;
-		case 1: rate = 88200; break; case 2: rate = 176400; break; case 3: rate = 192000; break; case 4: rate = 8000; break;
-		case 5: rate = 16000; break; case 6: rate = 22050; break; case 7: rate = 24000; break; case 8: rate = 32000; break;
-		case 9: rate = 44100; break; case 10: rate = 48000; break; case 11: rate = 96000; break;
-		case 12: rate = br.get(8) * 1000u; break;
-		case 13: rate = br.get(16); break;
-		case 14: rate = br.get(16) * 10u; break;
-		default: M.status = DEC_BAD_HEADER; meta[f] = M; return;
-	}
-	{   // CRC-8 over the header bytes (crc.c:39-76)
-		const uint32_t nb = (br.pos - start) >> 3;
-		const uint8_t *p = frames + off;
-		uint32_t crc = 0;
-		for(uint32_t b = 0; b < nb && b < len; b++) {
-			crc ^= p[b];
-			for(int j = 0; j < 8; j++) crc = (crc & 0x80u) ? ((crc << 1) ^ 0x07u) & 0xffu : (crc << 1) & 0xffu;
-		}
-		if(br.get(8) != crc) { M.status = DEC_CRC8; meta[f] = M; return; }
-	}
-	uint32_t channels, ca;
-	if(ca_code < 8) { channels = ca_code + 1; ca = 0; }
-	else if(ca_code <= 10) { channels = 2; ca = ca_code - 7; }
-	else { M.status = DEC_BAD_HEADER; meta[f] = M; return; }
-	uint32_t bps;
-	switch(bps_code) {
-		case 0: bps = (uint32_t)P.bps; break;
-		case 1: bps = 8; break; case 2: bps = 12; break; case 4: bps = 16; break;
-		case 5: bps = 20; break; case 6: bps = 24; break; case 7: bps = 32; break;
-		default: M.status = DEC_BAD_HEADER; meta[f] = M; return;
-	}
-	M.blocksize = blocksize; M.channel_assignment = ca; M.channels = channels; M.frame_number_lo = (uint32_t)number; M.variable = variable; M.sample_rate = rate;
+	br.init(frames + off, len, 8 * hr.bytes);
+	const uint32_t start = br.pos - 8 * hr.bytes;
+	M.blocksize = blocksize; M.channel_assignment = ca; M.channels = channels; M.frame_number_lo = (uint32_t)fh.number; M.variable = fh.variable; M.sample_rate = fh.sample_rate;
 	if(blocksize > (uint32_t)P.blocksize || channels != (uint32_t)P.channels || bps != (uint32_t)P.bps || bps > 24) {
 		M.status = (bps > 24) ? DEC_UNSUPPORTED : DEC_MISMATCH;
 		meta[f] = M;
@@ -784,18 +692,6 @@ __global__ void __launch_bounds__(256) k_dec_pack(const int32_t *__restrict__ pc
 }
 
 // ================================================================ k_dec_crc
-// GF(2)[x] multiply mod x^16+x^15+x^2+1
-__device__ __forceinline__ uint32_t dec_gf16_mul(uint32_t a, uint32_t b)
-{
-	uint32_t r = 0;
-#pragma unroll
-	for(int i = 15; i >= 0; i--) {
-		r = (r & 0x8000u) ? ((r << 1) ^ 0x8005u) & 0xffffu : (r << 1);
-		if((b >> i) & 1u) r ^= a;
-	}
-	return r;
-}
-
 // Device table of the CRC-16 pass (uint16): [0, 1024) slicing-by-4 tables T[k][b] = CRC of byte b followed by k zero bytes;
 // [1024 + (Lw - 1) * 5 + s] = x^(32 Lw 2^s) mod (x^16+x^15+x^2+1) for Lw = 1..kDecCrcLw, s < 5: the multipliers that combine
 // the 32 lane CRCs of a frame (crc(A || B) = crc(A) x^|B| + crc(B), init 0).
@@ -805,26 +701,16 @@ __global__ void k_dec_crc_tables(uint16_t *__restrict__ tab)
 {
 	const int t = blockIdx.x * blockDim.x + threadIdx.x;
 	if(t < 256) {
-		uint32_t c = (uint32_t)t << 8;
-#pragma unroll
-		for(int j = 0; j < 8; j++) c = (c & 0x8000u) ? ((c << 1) ^ 0x8005u) & 0xffffu : (c << 1) & 0xffffu;
-		uint32_t prev = c;
-		tab[t] = (uint16_t)c;
+		uint32_t prev = crc16_entry((uint32_t)t);
+		tab[t] = (uint16_t)prev;
 		for(int k = 1; k < 4; k++) {
-			// one more zero byte: shift the 16-bit state through 8 zero bits
-			for(int j = 0; j < 8; j++) prev = (prev & 0x8000u) ? ((prev << 1) ^ 0x8005u) & 0xffffu : (prev << 1) & 0xffffu;
+			prev = ((prev << 8) & 0xffffu) ^ crc16_entry(prev >> 8);  // one more zero byte
 			tab[k * 256 + t] = (uint16_t)prev;
 		}
 	}
 	if(t < kDecCrcLw * 5) {
 		const uint32_t Lw = (uint32_t)(t / 5) + 1u;
-		unsigned long long e = (32ull * Lw) << (t % 5);
-		uint32_t m = 1, bb = 2;  // x^e by square and multiply
-		while(e) {
-			if(e & 1ull) m = dec_gf16_mul(m, bb);
-			bb = dec_gf16_mul(bb, bb);
-			e >>= 1;
-		}
+		const uint32_t m = gf16_xpow((32ull * Lw) << (t % 5));
 		tab[1024 + t] = (uint16_t)m;
 	}
 }
@@ -881,20 +767,9 @@ __global__ void __launch_bounds__(128) k_dec_crc(const uint8_t *__restrict__ fra
 	}
 #pragma unroll
 	for(int s = 0; s < 5; s++) {
-		uint32_t m;
-		if(Lw <= (uint32_t)kDecCrcLw) m = __ldg(&crc_tab[1024 + (Lw - 1) * 5 + s]);
-		else {
-			unsigned long long e = (32ull * Lw) << s;
-			uint32_t bb = 2;
-			m = 1;
-			while(e) {
-				if(e & 1ull) m = dec_gf16_mul(m, bb);
-				bb = dec_gf16_mul(bb, bb);
-				e >>= 1;
-			}
-		}
+		const uint32_t m = Lw <= (uint32_t)kDecCrcLw ? __ldg(&crc_tab[1024 + (Lw - 1) * 5 + s]) : gf16_xpow((32ull * Lw) << s);
 		const uint32_t other = __shfl_down_sync(0xffffffffu, crc, 1 << s);
-		if((lane & ((2 << s) - 1)) == 0) crc = dec_gf16_mul(crc, m) ^ other;
+		if((lane & ((2 << s) - 1)) == 0) crc = gf16_mul(crc, m) ^ other;
 	}
 	if(lane == 0) {
 		const uint32_t want = ((uint32_t)p[nbytes] << 8) | p[nbytes + 1];

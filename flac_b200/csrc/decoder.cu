@@ -599,7 +599,7 @@ int fb200_decode_files_index(fb200_decoder *d, const uint8_t *data, uint64_t nby
 		const uint64_t fend = file_offsets[f + 1];
 		FrameHeader fh;
 		memset(&fh, 0, sizeof fh);
-		if(!parse_frame_header(data + pos, (size_t)(fend - pos), s, fh)) continue;
+		if(parse_frame_header(data + pos, (size_t)(fend - pos), s.sample_rate, s.bits_per_sample, fh).status != DEC_OK) continue;
 		if(fh.channels != s.channels || fh.bps != s.bits_per_sample || fh.blocksize > s.max_blocksize) continue;
 		Cand c;
 		c.begin = pos;

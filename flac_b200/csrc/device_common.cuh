@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #include "fb200_internal.h"
+#include "flac_frame.cuh"
 #include "glibc_log_data.h"
 
 namespace fb200 {
@@ -336,82 +337,17 @@ __device__ __forceinline__ uint32_t frame_number_of(const EncK &P, int blk)
 	return P.first_frame + (P.file_blocks ? gblk % (uint32_t)P.file_blocks : gblk);
 }
 
-// frame header layout (stream_encoder_framing.c:245-391)
-struct FrameHdr {
-	uint32_t bs_code, bs_hint, sr_code, sr_hint, utf8_len, bits;
-};
-
-__device__ __forceinline__ FrameHdr frame_header_layout(const EncK &P, int bs, uint32_t frame_number)
-{
-	FrameHdr H;
-	H.bs_hint = 0; H.sr_hint = 0;
-	switch(bs) {
-		case 192: H.bs_code = 1; break; case 576: H.bs_code = 2; break; case 1152: H.bs_code = 3; break;
-		case 2304: H.bs_code = 4; break; case 4608: H.bs_code = 5; break; case 256: H.bs_code = 8; break;
-		case 512: H.bs_code = 9; break; case 1024: H.bs_code = 10; break; case 2048: H.bs_code = 11; break;
-		case 4096: H.bs_code = 12; break; case 8192: H.bs_code = 13; break; case 16384: H.bs_code = 14; break;
-		case 32768: H.bs_code = 15; break;
-		default: H.bs_code = H.bs_hint = (bs <= 0x100) ? 6 : 7; break;
-	}
-	switch(P.sample_rate) {
-		case 88200: H.sr_code = 1; break; case 176400: H.sr_code = 2; break; case 192000: H.sr_code = 3; break;
-		case 8000: H.sr_code = 4; break; case 16000: H.sr_code = 5; break; case 22050: H.sr_code = 6; break;
-		case 24000: H.sr_code = 7; break; case 32000: H.sr_code = 8; break; case 44100: H.sr_code = 9; break;
-		case 48000: H.sr_code = 10; break; case 96000: H.sr_code = 11; break;
-		default:
-			if(P.sample_rate <= 255000 && P.sample_rate % 1000 == 0) H.sr_code = H.sr_hint = 12;
-			else if(P.sample_rate <= 655350 && P.sample_rate % 10 == 0) H.sr_code = H.sr_hint = 14;
-			else if(P.sample_rate <= 0xffff) H.sr_code = H.sr_hint = 13;
-			else H.sr_code = 0;
-			break;
-	}
-	if(frame_number < 0x80) H.utf8_len = 1;
-	else if(frame_number < 0x800) H.utf8_len = 2;
-	else if(frame_number < 0x10000) H.utf8_len = 3;
-	else if(frame_number < 0x200000) H.utf8_len = 4;
-	else if(frame_number < 0x4000000) H.utf8_len = 5;
-	else H.utf8_len = 6;
-	H.bits = 32 + 8 * H.utf8_len + (H.bs_hint ? (H.bs_hint == 6 ? 8 : 16) : 0) + (H.sr_hint ? (H.sr_hint == 12 ? 8 : 16) : 0) + 8;
-	return H;
-}
-
 // one thread writes the frame header and its CRC-8 at bit 0 of the zeroed word buffer `words`
 __device__ __forceinline__ void put_frame_header(const EncK &P, uint32_t *words, int bs, uint32_t frame_number, int ca, const FrameHdr &H)
 {
-	BitPut bw;
-	bw.init(words, 0);
-	uint32_t ca_code;
-	switch(ca) { case 0: ca_code = (uint32_t)P.channels - 1; break; case 1: ca_code = 8; break; case 2: ca_code = 9; break; default: ca_code = 10; break; }
-	uint32_t bps_code;
-	switch(P.bps) { case 8: bps_code = 1; break; case 12: bps_code = 2; break; case 16: bps_code = 4; break; case 20: bps_code = 5; break; case 24: bps_code = 6; break; case 32: bps_code = 7; break; default: bps_code = 0; break; }
-	bw.put(0x3ffe, 14); bw.put(0, 1); bw.put(0, 1);
-	bw.put(H.bs_code, 4); bw.put(H.sr_code, 4); bw.put(ca_code, 4); bw.put(bps_code, 3); bw.put(0, 1);
-	// UTF-8 style frame number (bitwriter.c:832-933)
-	const uint32_t v = frame_number;
-	switch(H.utf8_len) {
-		case 1: bw.put(v, 8); break;
-		case 2: bw.put(0xC0 | (v >> 6), 8); break;
-		case 3: bw.put(0xE0 | (v >> 12), 8); break;
-		case 4: bw.put(0xF0 | (v >> 18), 8); break;
-		case 5: bw.put(0xF8 | (v >> 24), 8); break;
-		default: bw.put(0xFC | (v >> 30), 8); break;
+	const uint32_t cac = ca_code(ca, P.channels), bpsc = bps_code(P.bps), nb = (H.bits >> 3) - 1;  // nb: bytes in front of the CRC-8
+	uint32_t crc = 0, w = 0;
+	for(uint32_t b = 0; b <= nb; b++) {
+		const uint32_t byte = b < nb ? frame_header_byte(H, bs, P.sample_rate, frame_number, cac, bpsc, (int)b) : crc;
+		crc = crc8_byte(crc, byte);
+		w |= byte << (24 - 8 * (b & 3));
+		if((b & 3) == 3 || b == nb) { words[b >> 2] = w; w = 0; }
 	}
-	for(int k = (int)H.utf8_len - 2; k >= 0; k--) bw.put(0x80 | ((v >> (6 * k)) & 0x3F), 8);
-	if(H.bs_hint) bw.put((uint32_t)bs - 1, H.bs_hint == 6 ? 8 : 16);
-	if(H.sr_hint == 12) bw.put((uint32_t)P.sample_rate / 1000, 8);
-	else if(H.sr_hint == 13) bw.put((uint32_t)P.sample_rate, 16);
-	else if(H.sr_hint == 14) bw.put((uint32_t)P.sample_rate / 10, 16);
-	bw.finish();
-	// CRC-8, poly 0x07 (crc.c:39-76), over the header bytes written so far
-	const uint32_t nb = (H.bits - 8) >> 3;
-	uint32_t crc = 0;
-	for(uint32_t b = 0; b < nb; b++) {
-		crc ^= (words[b >> 2] >> (24 - 8 * (b & 3))) & 0xffu;
-		for(int j = 0; j < 8; j++) crc = (crc & 0x80u) ? ((crc << 1) ^ 0x07u) & 0xffu : (crc << 1) & 0xffu;
-	}
-	bw.init(words, H.bits - 8);
-	bw.put(crc, 8);
-	bw.finish();
 }
 
 // bits of a subframe header + warm-up + predictor description (everything in front of the residual)
@@ -454,18 +390,6 @@ __device__ __forceinline__ void put_subframe_header(uint32_t *words, uint32_t bi
 		bw.put((uint32_t)pl->porder, kRiceOrderLen);
 	}
 	bw.finish();
-}
-
-// GF(2)[x] multiply mod x^16+x^15+x^2+1 (CRC-16 poly 0x8005, crc.c:78)
-__device__ __forceinline__ uint32_t gf16_mul(uint32_t a, uint32_t b)
-{
-	uint32_t r = 0;
-#pragma unroll
-	for(int i = 15; i >= 0; i--) {
-		r = (r & 0x8000u) ? ((r << 1) ^ 0x8005u) & 0xffffu : (r << 1);
-		if((b >> i) & 1u) r ^= a;
-	}
-	return r;
 }
 
 // x^(2^j) mod (x^16+x^15+x^2+1) for j = 0..14 (x has order 32767, so x^(2^15) = x and the table is periodic);

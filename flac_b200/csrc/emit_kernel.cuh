@@ -36,9 +36,7 @@ namespace fb200 {
 __global__ void k_crc16_tables(uint16_t *__restrict__ tab)
 {
 	const int b = threadIdx.x;
-	uint32_t c = (uint32_t)b << 8;
-#pragma unroll
-	for(int j = 0; j < 8; j++) c = (c & 0x8000u) ? ((c << 1) ^ 0x8005u) & 0xffffu : (c << 1) & 0xffffu;
+	const uint32_t c = crc16_entry((uint32_t)b);
 	tab[b] = (uint16_t)c;
 	__syncthreads();
 	uint32_t prev = c;
@@ -49,10 +47,7 @@ __global__ void k_crc16_tables(uint16_t *__restrict__ tab)
 	// combine multipliers: tab[1024 + (Lw >> 1) * 9 + s] = x^(32 Lw 2^s) mod (x^16+x^15+x^2+1) for odd Lw < 64, s < 9
 	for(int idx = b; idx < kCrcLwRows * 9; idx += blockDim.x) {
 		const uint32_t Lw = 2u * (uint32_t)(idx / 9) + 1u;
-		unsigned long long e = (32ull * Lw) << (idx % 9);
-		uint32_t m = 1;
-		for(int j = 0; e; j++, e >>= 1)
-			if(e & 1ull) m = gf16_mul(m, kCrcXPow2[j % 15]);
+		const uint32_t m = gf16_xpow((32ull * Lw) << (idx % 9));
 		tab[1024 + idx] = (uint16_t)m;
 	}
 	__syncthreads();
@@ -158,89 +153,15 @@ __device__ __forceinline__ uint32_t emit3_frame_header(const EncK &P, int blk, i
 {
 	const int bs = P.bs;
 	const uint32_t frame_number = frame_number_of(P, blk);
-	uint32_t bs_code, bs_hint = 0, sr_code, sr_hint = 0;
-	switch(bs) {
-		case 192: bs_code = 1; break; case 576: bs_code = 2; break; case 1152: bs_code = 3; break;
-		case 2304: bs_code = 4; break; case 4608: bs_code = 5; break; case 256: bs_code = 8; break;
-		case 512: bs_code = 9; break; case 1024: bs_code = 10; break; case 2048: bs_code = 11; break;
-		case 4096: bs_code = 12; break; case 8192: bs_code = 13; break; case 16384: bs_code = 14; break;
-		case 32768: bs_code = 15; break;
-		default: bs_code = bs_hint = (bs <= 0x100) ? 6 : 7; break;
-	}
-	switch(P.sample_rate) {
-		case 88200: sr_code = 1; break; case 176400: sr_code = 2; break; case 192000: sr_code = 3; break;
-		case 8000: sr_code = 4; break; case 16000: sr_code = 5; break; case 22050: sr_code = 6; break;
-		case 24000: sr_code = 7; break; case 32000: sr_code = 8; break; case 44100: sr_code = 9; break;
-		case 48000: sr_code = 10; break; case 96000: sr_code = 11; break;
-		default:
-			if(P.sample_rate <= 255000 && P.sample_rate % 1000 == 0) sr_code = sr_hint = 12;
-			else if(P.sample_rate <= 655350 && P.sample_rate % 10 == 0) sr_code = sr_hint = 14;
-			else if(P.sample_rate <= 0xffff) sr_code = sr_hint = 13;
-			else sr_code = 0;
-			break;
-	}
-	uint32_t utf8_len;
-	if(frame_number < 0x80) utf8_len = 1;
-	else if(frame_number < 0x800) utf8_len = 2;
-	else if(frame_number < 0x10000) utf8_len = 3;
-	else if(frame_number < 0x200000) utf8_len = 4;
-	else if(frame_number < 0x4000000) utf8_len = 5;
-	else utf8_len = 6;
-	const uint32_t header_bits = 32 + 8 * utf8_len + (bs_hint ? (bs_hint == 6 ? 8 : 16) : 0) + (sr_hint ? (sr_hint == 12 ? 8 : 16) : 0) + 8;
+	const FrameHdr H = frame_header_layout(bs, P.sample_rate, frame_number);
 	if(build) {
-		// one header byte per lane; CRC-8 (poly 0x07, crc.c:39-76) of the whole header from per-byte CRCs weighted by
-		// x^(8 * bytes behind) -- no serial loop over the header
-		const int nb8 = (int)(header_bits >> 3);  // bytes including the CRC-8
-		const int pos_bs = 4 + (int)utf8_len;
-		const int bs_bytes = bs_hint ? (bs_hint == 6 ? 1 : 2) : 0;
-		const int pos_sr = pos_bs + bs_bytes;
-		const int sr_bytes = sr_hint ? (sr_hint == 12 ? 1 : 2) : 0;
-		uint32_t ca_code;
-		switch(ca) { case 0: ca_code = (uint32_t)P.channels - 1; break; case 1: ca_code = 8; break; case 2: ca_code = 9; break; default: ca_code = 10; break; }
-		uint32_t bps_code;
-		switch(P.bps) { case 8: bps_code = 1; break; case 12: bps_code = 2; break; case 16: bps_code = 4; break; case 20: bps_code = 5; break; case 24: bps_code = 6; break; case 32: bps_code = 7; break; default: bps_code = 0; break; }
-		const uint32_t v = frame_number;
-		uint32_t byte = 0;
+		// one header byte per lane; CRC-8 of the whole header from per-byte CRCs weighted by x^(8 * bytes behind) -- no serial
+		// loop over the header
+		const int nb8 = (int)(H.bits >> 3);  // bytes including the CRC-8
 		const int i = lane;
-		if(i == 0) byte = 0xff;                                   // sync 0x3ffe, reserved 0, fixed-blocksize stream
-		else if(i == 1) byte = 0xf8;
-		else if(i == 2) byte = (bs_code << 4) | sr_code;
-		else if(i == 3) byte = (ca_code << 4) | (bps_code << 1);
-		else if(i < pos_bs) {                                     // UTF-8 style frame number (bitwriter.c:832-933)
-			const int j = i - 4;
-			if(j == 0) {
-				switch(utf8_len) {
-					case 1: byte = v; break;
-					case 2: byte = 0xC0 | (v >> 6); break;
-					case 3: byte = 0xE0 | (v >> 12); break;
-					case 4: byte = 0xF0 | (v >> 18); break;
-					case 5: byte = 0xF8 | (v >> 24); break;
-					default: byte = 0xFC | (v >> 30); break;
-				}
-			}
-			else byte = 0x80 | ((v >> (6 * ((int)utf8_len - 1 - j))) & 0x3F);
-		}
-		else if(i < pos_sr) byte = ((uint32_t)bs - 1) >> (8 * (bs_bytes - 1 - (i - pos_bs)));
-		else if(i < nb8 - 1) {
-			const uint32_t sv = sr_hint == 12 ? (uint32_t)P.sample_rate / 1000 : sr_hint == 13 ? (uint32_t)P.sample_rate : (uint32_t)P.sample_rate / 10;
-			byte = sv >> (8 * (sr_bytes - 1 - (i - pos_sr)));
-		}
-		byte &= 0xffu;
+		uint32_t byte = frame_header_byte(H, bs, P.sample_rate, frame_number, ca_code(ca, P.channels), bps_code(P.bps), i);
 		uint32_t c = 0;
-		if(i < nb8 - 1) {
-			c = byte;
-#pragma unroll
-			for(int j = 0; j < 8; j++) c = (c & 0x80u) ? ((c << 1) ^ 0x07u) & 0xffu : (c << 1) & 0xffu;
-			// times x^(8 * (nb8 - 2 - i)) in GF(2)[x] / (x^8 + x^2 + x + 1)
-			const uint32_t wgt = kCrc8XPow8[nb8 - 2 - i];
-			uint32_t r = 0;
-#pragma unroll
-			for(int j = 7; j >= 0; j--) {
-				r = (r & 0x80u) ? ((r << 1) ^ 0x07u) & 0xffu : (r << 1) & 0xffu;
-				if((wgt >> j) & 1u) r ^= c;
-			}
-			c = r;
-		}
+		if(i < nb8 - 1) c = gf8_mul(crc8_byte(0, byte), kCrc8XPow8[nb8 - 2 - i]);
 #pragma unroll
 		for(int o = 16; o > 0; o >>= 1) c ^= __shfl_xor_sync(0xffffffffu, c, o);
 		if(i == nb8 - 1) byte = c;
@@ -251,7 +172,7 @@ __device__ __forceinline__ uint32_t emit3_frame_header(const EncK &P, int blk, i
 		if((i & 3) == 0 && i < 16) hdr[i >> 2] = w;  // big-endian words, left aligned
 	}
 
-	return header_bits;
+	return H.bits;
 }
 
 // The end of a frame that sits in `words` with its END word aligned (s0 leading pad bytes, CRC-16 slot at word wend): CRC-16,

@@ -691,12 +691,7 @@ __global__ void __launch_bounds__(256) k_emit(EncK P, const int32_t *__restrict_
 	__shared__ int s_ca;
 
 	for(int i = tid; i < P.slot_words; i += nthr) words[i] = 0;
-	{   // CRC-16 table entry (crc.c:78-342)
-		uint32_t c = (uint32_t)tid << 8;
-#pragma unroll
-		for(int j = 0; j < 8; j++) c = (c & 0x8000u) ? ((c << 1) ^ 0x8005u) : (c << 1);
-		s_crctab[tid] = (uint16_t)c;
-	}
+	s_crctab[tid] = (uint16_t)crc16_entry((uint32_t)tid);
 	const SubframePlan *bp = plans + (size_t)blk * P.nsig;
 	if(tid == 0) s_ca = channel_assignment(P, bp, blkflags[blk]);
 	__syncthreads();
@@ -704,7 +699,7 @@ __global__ void __launch_bounds__(256) k_emit(EncK P, const int32_t *__restrict_
 	const uint32_t frame_number = frame_number_of(P, blk);
 
 	// ---- frame header (stream_encoder_framing.c:245-391), thread 0
-	const FrameHdr H = frame_header_layout(P, bs, frame_number);
+	const FrameHdr H = frame_header_layout(bs, P.sample_rate, frame_number);
 	if(tid == 0) put_frame_header(P, words, bs, frame_number, ca, H);
 	__syncthreads();
 
@@ -830,12 +825,7 @@ __global__ void __launch_bounds__(256) k_emit(EncK P, const int32_t *__restrict_
 		s_crc[tid] = crc;
 		if(tid == 0) {
 			// x^(8L) mod P by square-and-multiply, then repeated squaring for the tree levels
-			uint32_t result = 1, base = 2, e = 8 * L;
-			while(e) {
-				if(e & 1) result = gf16_mul(result, base);
-				base = gf16_mul(base, base);
-				e >>= 1;
-			}
+			uint32_t result = gf16_xpow(8ull * L);
 			for(int s = 0; s < 8; s++) { s_mlev[s] = result; result = gf16_mul(result, result); }
 		}
 		__syncthreads();

@@ -1,4 +1,4 @@
-// flac_parse.cu -- host-side parsing of .flac containers and frame headers (flac_parse.h). No device code.
+// flac_parse.cu -- host-side parsing of .flac containers (flac_parse.h). No device code.
 #include <stdio.h>
 #include <string.h>
 #include <strings.h>
@@ -8,63 +8,6 @@
 #include "flac_parse.h"
 
 namespace fb200 {
-
-static uint8_t crc8_update(uint8_t crc, uint8_t byte)
-{
-	uint32_t c = crc ^ byte;
-	for(int j = 0; j < 8; j++) c = (c & 0x80) ? ((c << 1) ^ 0x07) : (c << 1);
-	return (uint8_t)c;
-}
-
-uint32_t parse_frame_header(const uint8_t *p, size_t avail, const FLAC__StreamMetadata_StreamInfo &si, FrameHeader &fe)
-{
-	if(avail < 6 || p[0] != 0xFF || (p[1] & 0xFE) != 0xF8) return 0;
-	fe.variable = p[1] & 1;
-	const uint32_t bs_code = p[2] >> 4, sr_code = p[2] & 15, ca_code = p[3] >> 4, bps_code = (p[3] >> 1) & 7;
-	if(p[3] & 1) return 0;
-	if(bs_code == 0 || sr_code == 15 || ca_code > 10 || bps_code == 3) return 0;
-	size_t pos = 4;
-	uint64_t number;
-	{
-		const uint32_t first = p[pos++];
-		int n;
-		if(!(first & 0x80)) { number = first; n = 0; }
-		else if((first & 0xE0) == 0xC0) { number = first & 0x1F; n = 1; }
-		else if((first & 0xF0) == 0xE0) { number = first & 0x0F; n = 2; }
-		else if((first & 0xF8) == 0xF0) { number = first & 0x07; n = 3; }
-		else if((first & 0xFC) == 0xF8) { number = first & 0x03; n = 4; }
-		else if((first & 0xFE) == 0xFC) { number = first & 0x01; n = 5; }
-		else if(first == 0xFE && fe.variable) { number = 0; n = 6; }
-		else return 0;
-		if(pos + n + 3 > avail) return 0;
-		for(int k = 0; k < n; k++) {
-			if((p[pos] & 0xC0) != 0x80) return 0;
-			number = (number << 6) | (p[pos++] & 0x3F);
-		}
-	}
-	switch(bs_code) {
-		case 1: fe.blocksize = 192; break;
-		case 2: case 3: case 4: case 5: fe.blocksize = 576u << (bs_code - 2); break;
-		case 6: fe.blocksize = p[pos++] + 1u; break;
-		case 7: fe.blocksize = (((uint32_t)p[pos] << 8) | p[pos + 1]) + 1u; pos += 2; break;
-		default: fe.blocksize = 256u << (bs_code - 8); break;
-	}
-	static const uint32_t rates[12] = {0, 88200, 176400, 192000, 8000, 16000, 22050, 24000, 32000, 44100, 48000, 96000};
-	if(sr_code < 12) fe.sample_rate = sr_code ? rates[sr_code] : si.sample_rate;
-	else if(sr_code == 12) fe.sample_rate = p[pos++] * 1000u;
-	else { const uint32_t v = ((uint32_t)p[pos] << 8) | p[pos + 1]; pos += 2; fe.sample_rate = sr_code == 13 ? v : v * 10; }
-	if(pos + 1 > avail) return 0;
-	uint8_t crc = 0;
-	for(size_t i = 0; i < pos; i++) crc = crc8_update(crc, p[i]);
-	if(crc != p[pos]) return 0;
-	fe.crc8 = crc;
-	fe.number = number;
-	fe.channels = ca_code < 8 ? ca_code + 1 : 2;
-	fe.ca = ca_code < 8 ? 0 : ca_code - 7;
-	static const uint32_t bpss[8] = {0, 8, 12, 0, 16, 20, 24, 32};
-	fe.bps = bps_code ? bpss[bps_code] : si.bits_per_sample;
-	return (uint32_t)pos + 1;
-}
 
 void get_streaminfo(const uint8_t *b, FLAC__StreamMetadata_StreamInfo &s)
 {

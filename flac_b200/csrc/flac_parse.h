@@ -1,4 +1,4 @@
-// flac_parse.h -- host-side parsing of .flac containers, metadata blocks and frame headers: the one reader of each format rule
+// flac_parse.h -- host-side parsing of .flac containers and metadata blocks: the one reader of each format rule
 // for the FLAC__stream_decoder_* shell (stream_api.cu), the batch decoders and every batch-file path that reads FLAC metadata.
 #pragma once
 
@@ -10,21 +10,9 @@
 #include <vector>
 
 #include "../../include/flac_b200_stream.h"
+#include "flac_frame.cuh"
 
 namespace fb200 {
-
-// The facts of one frame header (stream_decoder.c:2624-2947).
-struct FrameHeader {
-	uint32_t blocksize;
-	uint64_t number;      // frame or sample number from the header
-	uint32_t variable;    // blocking strategy bit
-	uint32_t sample_rate, channels, bps, ca;
-	uint8_t crc8;
-};
-
-// Parses the frame header at p (avail bytes readable) incl. its CRC-8; sample rate / bps code 0 take STREAMINFO's values.
-// Returns the header length in bytes, or 0 when there is no valid header at p.
-uint32_t parse_frame_header(const uint8_t *p, size_t avail, const FLAC__StreamMetadata_StreamInfo &si, FrameHeader &fh);
 
 // The 34-byte STREAMINFO body (format.c:65-73) into its fields.
 void get_streaminfo(const uint8_t *body, FLAC__StreamMetadata_StreamInfo &si);

@@ -99,24 +99,6 @@ struct MD5 {
 	}
 };
 
-uint8_t g_crc8[256];
-uint16_t g_crc16[256];
-bool g_crc_ready = false;
-void crc_init()
-{
-	if(g_crc_ready) return;
-	for(uint32_t i = 0; i < 256; i++) {
-		uint32_t c8 = i, c16 = i << 8;
-		for(int j = 0; j < 8; j++) {
-			c8 = (c8 & 0x80) ? ((c8 << 1) ^ 0x07) : (c8 << 1);
-			c16 = (c16 & 0x8000) ? ((c16 << 1) ^ 0x8005) : (c16 << 1);
-		}
-		g_crc8[i] = (uint8_t)c8;
-		g_crc16[i] = (uint16_t)c16;
-	}
-	g_crc_ready = true;
-}
-
 struct ByteWriter {
 	std::vector<uint8_t> v;
 	void u(uint64_t val, int nbytes) { for(int i = nbytes - 1; i >= 0; i--) v.push_back((uint8_t)(val >> (8 * i))); }
@@ -349,7 +331,6 @@ extern "C" {
 
 FLAC__StreamEncoder *FLAC__stream_encoder_new(void)
 {
-	crc_init();
 	FLAC__StreamEncoder *e = (FLAC__StreamEncoder *)calloc(1, sizeof *e);
 	if(!e) return nullptr;
 	e->protected_ = new FLAC__StreamEncoderProtected();
@@ -974,7 +955,7 @@ static bool dec_build_index(FLAC__StreamDecoder *d)
 		FrameIndexEntry fe;
 		memset(&fe, 0, sizeof fe);
 		const size_t pos = (size_t)cand[i];
-		if(!fb200::parse_frame_header(a + pos, n - pos, q->si, fe)) continue;
+		if(fb200::parse_frame_header(a + pos, n - pos, q->si.sample_rate, q->si.bits_per_sample, fe).status != fb200::DEC_OK) continue;
 		if(fe.channels != q->si.channels || fe.bps != q->si.bits_per_sample || fe.blocksize > (q->si.max_blocksize ? q->si.max_blocksize : 65535u)) continue;
 		fe.offset = pos; fe.length = 0;
 		q->index.push_back(fe);
@@ -1284,7 +1265,6 @@ extern "C" {
 
 FLAC__StreamDecoder *FLAC__stream_decoder_new(void)
 {
-	crc_init();
 	FLAC__StreamDecoder *d = (FLAC__StreamDecoder *)calloc(1, sizeof *d);
 	if(!d) return nullptr;
 	d->protected_ = new FLAC__StreamDecoderProtected();

@@ -471,18 +471,13 @@ __global__ void __launch_bounds__(kJoinThreads) k_join_tiled(EncK P, const int *
 	__shared__ uint32_t s_total;
 	__shared__ int s_ca, s_bad;
 	const int blk = blockIdx.x, tid = threadIdx.x, ch = P.channels;
-	if(tid < 256) {  // CRC-16 table entry (crc.c:78-342)
-		uint32_t cr = (uint32_t)tid << 8;
-#pragma unroll
-		for(int j = 0; j < 8; j++) cr = (cr & 0x8000u) ? ((cr << 1) ^ 0x8005u) : (cr << 1);
-		s_crctab[tid] = (uint16_t)cr;
-	}
+	if(tid < 256) s_crctab[tid] = (uint16_t)crc16_entry((uint32_t)tid);
 	if(tid < 5) s_hdr[tid] = 0;
 	__syncthreads();
 	if(tid == 0) {
 		const int ca = channel_assignment(P, plans + (size_t)blk * P.nsig, blkflags[blk]);
 		const uint32_t frame_number = frame_number_of(P, blk);
-		const FrameHdr H = frame_header_layout(P, P.bs, frame_number);
+		const FrameHdr H = frame_header_layout(P.bs, P.sample_rate, frame_number);
 		put_frame_header(P, s_hdr, P.bs, frame_number, ca, H);
 		uint32_t off = H.bits;
 		int bad = 0;
@@ -530,12 +525,7 @@ __global__ void __launch_bounds__(kJoinThreads) k_join_tiled(EncK P, const int *
 	}
 	{
 		// shift this run's CRC past the bytes behind it: x^(8 * behind) mod the CRC-16 polynomial, square and multiply
-		uint32_t e8 = 8u * (nbytes - min(nbytes, 4u * w1)), m = 1, b = 2;
-		while(e8) {
-			if(e8 & 1u) m = gf16_mul(m, b);
-			b = gf16_mul(b, b);
-			e8 >>= 1;
-		}
+		const uint32_t m = gf16_xpow(8u * (nbytes - min(nbytes, 4u * w1)));
 		crc = gf16_mul(crc, m);
 	}
 	crc = __reduce_xor_sync(0xffffffffu, crc);
